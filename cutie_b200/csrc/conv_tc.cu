@@ -38,6 +38,15 @@
 //     step go into a fresh accumulator that is then added to an fp32 total with round-to-nearest adds.
 //   * Epilogue: straight from the accumulator fragments (element-wise); bias, optional residual, optional ReLU; ReLU on
 //     the INPUT (the pre-activation blocks' conv(relu(x))) is applied by the producers for free.
+//   * FP16 operands (template parameter F16; cutie_conv_tc_f16, what CUDA autocast asks of a convolution): the same kernel,
+//     plan, tiles, epilogues and fp32 inputs / outputs, but the producers round pre(x) to fp16 (RN, one plane, no split),
+//     the weight image holds one fp16 [128 x 32] plane per (chunk, tap) (8 KB), and a (chunk, tap) step is TWO
+//     wgmma.m64n128k16.f32.f16.f16 per warpgroup instead of twelve tf32 ones.  A row of 32 channels is then 64 bytes, so
+//     both operands use K-major SWIZZLE_64B (8-row atoms of 512 B, 16-byte chunk index XOR address bits 7-8).  The row-shift
+//     argument above holds unchanged: the 64-byte swizzle is likewise applied to absolute address bits, every operand tile
+//     base (activation stages, weight stages, the second warpgroup's half) is 512-byte aligned, so the producers' pattern
+//     ((chunk ^ (row >> 1)) & 3 with row counted from the base) is the address-based one and a start shifted by r rows of
+//     64 bytes reads rows r.. of it.  The fresh-accumulator-per-step promotion is kept (DESIGN.md section 3.7).
 //
 // Warp roles (544 threads): warps 0-7 two MMA + epilogue warpgroups (output channels 0-63 / 64-127 of the tile), warps
 // 8-15 activation producers (global fp32 -> hi/lo -> swizzled smem, next chunk's loads in flight during the current
@@ -51,25 +60,33 @@ namespace {
 
 constexpr int CV_M = 128;                         // output channels per CTA
 constexpr int CV_KC = 32;                         // input channels per chunk
-constexpr int CV_A_BYTES = 2 * CV_M * 128;        // hi | lo planes of one (chunk, tap) weight block: 32768
 constexpr int CV_A_STAGES = 3;
 constexpr int CV_THREADS = 544;
 constexpr int CV_PROD = 256;
 constexpr int CV3_ROWS = 248;                     // 3x3: activation tile rows per stage (31 x 8: planes stay 1024-byte aligned)
 constexpr int CV1_ROWS = 128;                     // 1x1
+constexpr int CV_STAGING = 65 * 1024;             // the finished tile staged as fp32 [128][N | 1 <= 129] (66048 B), 1 KB aligned
+
+// operand precision: 3xTF32 = hi | lo planes of 128-byte rows (32 tf32); FP16 = one plane of 64-byte rows (32 f16)
+__host__ __device__ constexpr int cv_row_bytes(bool f16) { return f16 ? 64 : 128; }
+__host__ __device__ constexpr int cv_planes(bool f16) { return f16 ? 1 : 2; }
+__host__ __device__ constexpr int cv_a_bytes(bool f16) { return cv_planes(f16) * CV_M * cv_row_bytes(f16); }   // 32768 | 8192
+// activation stages (3x3: 2 x 248 rows, 1x1: 4 x 128 rows); the epilogue's staging buffer aliases them, so at least that
+__host__ __device__ constexpr int cv_x_bytes(int ks, bool f16) {
+  const int operands = (ks == 3 ? 2 * CV3_ROWS : 4 * CV1_ROWS) * cv_planes(f16) * cv_row_bytes(f16);
+  return operands > CV_STAGING ? operands : CV_STAGING;
+}
 
 struct ConvTail {
   unsigned long long a_full[CV_A_STAGES], a_empty[CV_A_STAGES], x_full[4], x_empty[4];
   int last[2];
 };
-constexpr int CV_X_BYTES3 = 2 * 2 * CV3_ROWS * 128;   // 3x3: 2 stages x (hi | lo) x 248 rows = 126976
-constexpr int CV_X_BYTES1 = 4 * 2 * CV1_ROWS * 128;   // 1x1: 4 stages x (hi | lo) x 128 rows = 131072
-constexpr int CV_SMEM3 = CV_X_BYTES3 + CV_A_STAGES * CV_A_BYTES + (int)sizeof(ConvTail) + 64;
-constexpr int CV_SMEM1 = CV_X_BYTES1 + CV_A_STAGES * CV_A_BYTES + (int)sizeof(ConvTail) + 64;
+// 3xTF32: 126976 (3x3) | 131072 (1x1) activation bytes + 3 x 32 KB weight stages; FP16: 66560 + 3 x 8 KB
+constexpr int cv_smem(int ks, bool f16) { return cv_x_bytes(ks, f16) + CV_A_STAGES * cv_a_bytes(f16) + (int)sizeof(ConvTail) + 64; }
 
 struct ConvTcParams {
   const float* x;
-  const unsigned char* wimg;   // [ceil(Cout / 128)][Cin / 32][taps][32768]
+  const unsigned char* wimg;   // [ceil(Cout / 128)][Cin / 32][taps][32768 (3xTF32) | 8192 (FP16)]
   const float* bias;           // [Cout] or null
   const float* z;              // residual, or null
   float* y;
@@ -101,20 +118,22 @@ struct ConvPart {              // one contiguous share of an output tile's input
   long long tile_lin;          // (nb, cot, tile) linearised: workspace / counter index
 };
 
-template <int KS>
+template <int KS, bool F16>
 __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcParams p) {
   constexpr int XROWS = KS == 3 ? CV3_ROWS : CV1_ROWS;
-  constexpr int XPLANE = XROWS * 128;
-  constexpr int XSTAGE = 2 * XPLANE;
+  constexpr int ROWB = cv_row_bytes(F16);                    // bytes per operand row (32 channels)
+  constexpr int XPLANE = XROWS * ROWB;
+  constexpr int XSTAGE = cv_planes(F16) * XPLANE;
   constexpr int XST = KS == 3 ? 2 : 4;                       // activation stages
+  constexpr int A_BYTES = cv_a_bytes(F16);
   constexpr int TAPS = KS * KS;
   constexpr int HALVES = KS == 3 ? 1 : 2;                    // producer threads per tile row (1x1: 16 channels each)
   constexpr int CPT = CV_KC / HALVES;                        // channels per producer thread and chunk
   constexpr int DEPTH = KS == 3 ? 1 : 2;                     // chunks of global loads in flight per producer thread
   extern __shared__ __align__(1024) unsigned char smem[];
   unsigned char* Xs = smem;
-  unsigned char* As = smem + XST * XSTAGE;
-  ConvTail& T = *reinterpret_cast<ConvTail*>(smem + XST * XSTAGE + CV_A_STAGES * CV_A_BYTES);
+  unsigned char* As = smem + cv_x_bytes(KS, F16);
+  ConvTail& T = *reinterpret_cast<ConvTail*>(As + CV_A_STAGES * A_BYTES);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int TWp = p.pitch;                                   // positions per local row of the 3x3 tile
   const int C = p.Cin / CV_KC;                               // input chunks per output tile
@@ -327,7 +346,18 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
           if (c < chunks) {
             const int s = xc % XST;
             mbar_wait(smem_u32(&T.x_empty[s]), ((xc / XST) & 1) ^ 1);
-            if (row_live) {
+            if (F16 && row_live) {
+              unsigned char* row = Xs + s * XSTAGE + r * ROWB;
+#pragma unroll
+              for (int k8 = 0; k8 < CPT / 8; ++k8) {
+                float f[8];
+#pragma unroll
+                for (int i = 0; i < 8; ++i) f[i] = p.relu_in ? fmaxf(v[d][8 * k8 + i], 0.f) : v[d][8 * k8 + i];
+                const int off = ((half * (CPT / 8) + k8) ^ ((r >> 1) & 3)) << 4;
+                *reinterpret_cast<uint4*>(row + off) =
+                    make_uint4(f16x2_rn(f[0], f[1]), f16x2_rn(f[2], f[3]), f16x2_rn(f[4], f[5]), f16x2_rn(f[6], f[7]));
+              }
+            } else if (row_live) {
               unsigned char* hi = Xs + s * XSTAGE + r * 128;
               unsigned char* lo = hi + XPLANE;
 #pragma unroll
@@ -355,13 +385,13 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
       int i = 0;
       for (int pi = 0; pi < nparts; ++pi) {
         const ConvPart& P = pi ? part1 : part0;
-        const unsigned char* wsrc = p.wimg + ((size_t)P.cot * C + P.c0) * TAPS * CV_A_BYTES;
+        const unsigned char* wsrc = p.wimg + ((size_t)P.cot * C + P.c0) * TAPS * A_BYTES;
         const int steps = (P.c1 - P.c0) * TAPS;
         for (int k = 0; k < steps; ++k, ++i) {
           const int s = i % CV_A_STAGES;
           mbar_wait(smem_u32(&T.a_empty[s]), ((i / CV_A_STAGES) & 1) ^ 1);
-          mbar_arrive_expect_tx(smem_u32(&T.a_full[s]), CV_A_BYTES);
-          bulk_g2s(smem_u32(As + s * CV_A_BYTES), wsrc + (size_t)k * CV_A_BYTES, CV_A_BYTES, smem_u32(&T.a_full[s]));
+          mbar_arrive_expect_tx(smem_u32(&T.a_full[s]), A_BYTES);
+          bulk_g2s(smem_u32(As + s * A_BYTES), wsrc + (size_t)k * A_BYTES, A_BYTES, smem_u32(&T.a_full[s]));
         }
       }
     }
@@ -385,17 +415,23 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
         for (int t = 0; t < TAPS; ++t, ++i) {
           const int s = i % CV_A_STAGES;
           mbar_wait(smem_u32(&T.a_full[s]), (i / CV_A_STAGES) & 1);
-          const uint32_t a_hi = smem_u32(As + s * CV_A_BYTES) + G * 64 * 128, a_lo = a_hi + CV_M * 128;
-          const uint32_t shift = KS == 3 ? (uint32_t)p.shift[t] * 128u : 0u;
+          const uint32_t a_hi = smem_u32(As + s * A_BYTES) + G * 64 * ROWB, a_lo = a_hi + CV_M * 128;
+          const uint32_t shift = KS == 3 ? (uint32_t)p.shift[t] * ROWB : 0u;
           wg_fence();
+          if constexpr (F16) {
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t da_hi = desc_sw128_kmajor(a_hi + ks * 32), da_lo = desc_sw128_kmajor(a_lo + ks * 32);
-            const uint64_t db_hi = desc_sw128_kmajor(xb_hi + shift + ks * 32);
-            const uint64_t db_lo = desc_sw128_kmajor(xb_lo + shift + ks * 32);
-            wgmma_tf32_n128(d, da_lo, db_hi, ks != 0 ? 1 : 0);
-            wgmma_tf32_n128(d, da_hi, db_lo, 1);
-            wgmma_tf32_n128(d, da_hi, db_hi, 1);
+            for (int ks = 0; ks < 2; ++ks)                     // k16 steps of 32 bytes
+              wgmma_f16_n128(d, desc_sw64_kmajor(a_hi + ks * 32), desc_sw64_kmajor(xb_hi + shift + ks * 32), ks);
+          } else {
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+              const uint64_t da_hi = desc_sw128_kmajor(a_hi + ks * 32), da_lo = desc_sw128_kmajor(a_lo + ks * 32);
+              const uint64_t db_hi = desc_sw128_kmajor(xb_hi + shift + ks * 32);
+              const uint64_t db_lo = desc_sw128_kmajor(xb_lo + shift + ks * 32);
+              wgmma_tf32_n128(d, da_lo, db_hi, ks != 0 ? 1 : 0);
+              wgmma_tf32_n128(d, da_hi, db_lo, 1);
+              wgmma_tf32_n128(d, da_hi, db_hi, 1);
+            }
           }
           wg_commit();
           wg_wait0();
@@ -530,10 +566,33 @@ __global__ void __launch_bounds__(256) conv_weight_image_kernel(const float* __r
   for (int i = 0; i < 4; ++i) v[i] = co < Cout ? w[((long long)co * Cin + c * CV_KC + 4 * k4 + i) * taps + t] : 0.f;
   const float4 h = make_float4(to_tf32(v[0]), to_tf32(v[1]), to_tf32(v[2]), to_tf32(v[3]));
   const float4 l = make_float4(to_tf32(v[0] - h.x), to_tf32(v[1] - h.y), to_tf32(v[2] - h.z), to_tf32(v[3] - h.w));
-  unsigned char* blk = img + (((size_t)cot * chunks + c) * taps + t) * CV_A_BYTES;
+  unsigned char* blk = img + (((size_t)cot * chunks + c) * taps + t) * cv_a_bytes(false);
   const int off = row * 128 + ((k4 ^ (row & 7)) << 4);
   *reinterpret_cast<float4*>(blk + off) = h;
   *reinterpret_cast<float4*>(blk + CV_M * 128 + off) = l;
+}
+
+// FP16 weight operand image: one fp16 [128 x 32] plane per (128-channel tile, chunk, tap), rows of 64 B in K-major
+// SWIZZLE_64B order; one thread per (output channel, chunk, tap, 16-byte piece of 8 channels)
+__global__ void __launch_bounds__(256) conv_weight_image_f16_kernel(const float* __restrict__ w, int Cout, int Cin, int taps,
+                                                                    unsigned char* __restrict__ img) {
+  const int chunks = Cin / CV_KC;
+  const long long total = (long long)((Cout + CV_M - 1) / CV_M * CV_M) * chunks * taps * 4;
+  const long long f = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (f >= total) return;
+  const int k8 = (int)(f & 3);
+  long long g = f >> 2;
+  const int row = (int)(g % CV_M); g /= CV_M;
+  const int t = (int)(g % taps); g /= taps;
+  const int c = (int)(g % chunks);
+  const int cot = (int)(g / chunks);
+  const int co = cot * CV_M + row;
+  float v[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] = co < Cout ? w[((long long)co * Cin + c * CV_KC + 8 * k8 + i) * taps + t] : 0.f;
+  unsigned char* blk = img + (((size_t)cot * chunks + c) * taps + t) * cv_a_bytes(true);
+  *reinterpret_cast<uint4*>(blk + row * 64 + ((k8 ^ ((row >> 1) & 3)) << 4)) =
+      make_uint4(f16x2_rn(v[0], v[1]), f16x2_rn(v[2], v[3]), f16x2_rn(v[4], v[5]), f16x2_rn(v[6], v[7]));
 }
 
 }  // namespace
@@ -542,21 +601,48 @@ __global__ void __launch_bounds__(256) conv_weight_image_kernel(const float* __r
 
 using namespace cutie;
 
-extern "C" int64_t cutie_conv_weight_image_bytes(int64_t Cout, int64_t Cin, int ksize) {
+// argument checks of the entry points below that share a body: the message names the entry point (`fn`) like CUTIE_REQUIRE
+#define CONV_REQUIRE(cond, what)                                                          \
+  do {                                                                                    \
+    if (!(cond)) return ::cutie::fail(-1, "%s: invalid argument: " what, fn);            \
+  } while (0)
+
+static int64_t conv_weight_image_bytes(int64_t Cout, int64_t Cin, int ksize, bool f16) {
   if (Cout < 1 || Cin < CV_KC || Cin % CV_KC || (ksize != 1 && ksize != 3)) return -1;
-  return ((Cout + CV_M - 1) / CV_M) * (Cin / CV_KC) * ksize * ksize * (int64_t)CV_A_BYTES;
+  return ((Cout + CV_M - 1) / CV_M) * (Cin / CV_KC) * ksize * ksize * (int64_t)cv_a_bytes(f16);
+}
+
+static int conv_weight_image(const char* fn, bool f16, const float* weight, int64_t Cout, int64_t Cin, int ksize, void* image,
+                             void* stream) {
+  CONV_REQUIRE(weight && image, "null argument");
+  CONV_REQUIRE(ksize == 1 || ksize == 3, "1x1 or 3x3");
+  CONV_REQUIRE(Cout >= 1 && Cin >= CV_KC && Cin % CV_KC == 0, "input channels must be a multiple of 32");
+  const int taps = ksize * ksize;
+  const long long pieces = (Cout + CV_M - 1) / CV_M * CV_M * (Cin / CV_KC) * taps;   // x 16-byte pieces per row
+  if (f16)
+    conv_weight_image_f16_kernel<<<(unsigned)((pieces * 4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        weight, (int)Cout, (int)Cin, taps, static_cast<unsigned char*>(image));
+  else
+    conv_weight_image_kernel<<<(unsigned)((pieces * 8 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        weight, (int)Cout, (int)Cin, taps, static_cast<unsigned char*>(image));
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : ::cutie::set_cuda_error(fn, e);
+}
+
+extern "C" int64_t cutie_conv_weight_image_bytes(int64_t Cout, int64_t Cin, int ksize) {
+  return conv_weight_image_bytes(Cout, Cin, ksize, false);
 }
 
 extern "C" int cutie_conv_weight_image(const float* weight, int64_t Cout, int64_t Cin, int ksize, void* image, void* stream) {
-  CUTIE_REQUIRE(weight && image, "null argument");
-  CUTIE_REQUIRE(ksize == 1 || ksize == 3, "1x1 or 3x3");
-  CUTIE_REQUIRE(Cout >= 1 && Cin >= CV_KC && Cin % CV_KC == 0, "input channels must be a multiple of 32");
-  const int taps = ksize * ksize;
-  const long long total = (Cout + CV_M - 1) / CV_M * CV_M * (Cin / CV_KC) * taps * 8;
-  conv_weight_image_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      weight, (int)Cout, (int)Cin, taps, static_cast<unsigned char*>(image));
-  CUTIE_CHECK_LAUNCH();
-  return 0;
+  return conv_weight_image(__func__, false, weight, Cout, Cin, ksize, image, stream);
+}
+
+extern "C" int64_t cutie_conv_weight_image_f16_bytes(int64_t Cout, int64_t Cin, int ksize) {
+  return conv_weight_image_bytes(Cout, Cin, ksize, true);
+}
+
+extern "C" int cutie_conv_weight_image_f16(const float* weight, int64_t Cout, int64_t Cin, int ksize, void* image, void* stream) {
+  return conv_weight_image(__func__, true, weight, Cout, Cin, ksize, image, stream);
 }
 
 // 3x3 spatial tile: TW | tile width (full rows when they fit), TH rows, N = round16(TH * (TW + 2)) <= 128 and
@@ -626,19 +712,20 @@ extern "C" int cutie_conv_plan(int64_t NB, int64_t Cin, int64_t Cout, int64_t H_
   return 0;
 }
 
-extern "C" int cutie_conv_tc(const float* x, const int64_t* x_strides, const void* weight_image, const float* bias,
-                             const float* residual, const int64_t* residual_strides, int64_t NB, int64_t Cin, int64_t Cout,
-                             int64_t H_in, int64_t W_in, int ksize, int stride, int relu_in, int relu_out, float* y,
-                             const int64_t* y_strides, int units_per_cta, float* workspace, int32_t* counters, void* stream) {
-  CUTIE_REQUIRE(x && x_strides && weight_image && y && y_strides, "null argument");
-  CUTIE_REQUIRE(residual == nullptr || residual_strides != nullptr, "residual needs strides");
-  CUTIE_REQUIRE((ksize == 3 || ksize == 1) && (stride == 1 || stride == 2), "3x3 (zero pad 1) or 1x1, stride 1 or 2");
-  CUTIE_REQUIRE(Cout >= 1 && Cin >= CV_KC && Cin % CV_KC == 0, "input channels must be a multiple of 32");
-  CUTIE_REQUIRE(NB >= 1 && NB <= 65535 && H_in >= 1 && W_in >= 1 && H_in * W_in < (1ll << 30), "bad geometry");
+template <bool F16>
+static int conv_tc_launch(const char* fn, const float* x, const int64_t* x_strides, const void* weight_image, const float* bias,
+                          const float* residual, const int64_t* residual_strides, int64_t NB, int64_t Cin, int64_t Cout,
+                          int64_t H_in, int64_t W_in, int ksize, int stride, int relu_in, int relu_out, float* y,
+                          const int64_t* y_strides, int units_per_cta, float* workspace, int32_t* counters, void* stream) {
+  CONV_REQUIRE(x && x_strides && weight_image && y && y_strides, "null argument");
+  CONV_REQUIRE(residual == nullptr || residual_strides != nullptr, "residual needs strides");
+  CONV_REQUIRE((ksize == 3 || ksize == 1) && (stride == 1 || stride == 2), "3x3 (zero pad 1) or 1x1, stride 1 or 2");
+  CONV_REQUIRE(Cout >= 1 && Cin >= CV_KC && Cin % CV_KC == 0, "input channels must be a multiple of 32");
+  CONV_REQUIRE(NB >= 1 && NB <= 65535 && H_in >= 1 && W_in >= 1 && H_in * W_in < (1ll << 30), "bad geometry");
   ConvPlan pl;
-  CUTIE_REQUIRE(conv_make_plan(NB, Cin, Cout, H_in, W_in, ksize, stride, units_per_cta, &pl) == 0, "no tile shape for this geometry");
-  CUTIE_REQUIRE(pl.q == pl.C || (workspace && counters), "shared tiles need the workspace and zeroed counters (cutie_conv_plan)");
-  CUTIE_REQUIRE(pl.ctas <= 0x7fffffff, "too many tiles");
+  CONV_REQUIRE(conv_make_plan(NB, Cin, Cout, H_in, W_in, ksize, stride, units_per_cta, &pl) == 0, "no tile shape for this geometry");
+  CONV_REQUIRE(pl.q == pl.C || (workspace && counters), "shared tiles need the workspace and zeroed counters (cutie_conv_plan)");
+  CONV_REQUIRE(pl.ctas <= 0x7fffffff, "too many tiles");
   ConvTcParams p;
   p.x = x; p.wimg = static_cast<const unsigned char*>(weight_image); p.bias = bias; p.z = residual; p.y = y;
   p.xs_n = x_strides[0]; p.xs_c = x_strides[1]; p.xs_p = x_strides[2];
@@ -674,18 +761,34 @@ extern "C" int cutie_conv_tc(const float* x, const int64_t* x_strides, const voi
   }
   p.q = pl.q; p.T = (int)pl.T; p.tiles = (int)pl.tiles; p.cots = (int)pl.cots; p.maxslots = pl.maxslots;
   p.ws = workspace; p.counters = counters;
-  CUTIE_REQUIRE(pl.T <= 0x7fffffff, "too many tiles");
-  static bool attr_done[64] = {};
+  CONV_REQUIRE(pl.T <= 0x7fffffff, "too many tiles");
+  static bool attr_done[64] = {};                            // (one per instantiation, i.e. per precision)
   if (first_use_on_device(attr_done)) {
-    cudaFuncSetAttribute(conv_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, CV_SMEM3);
-    cudaFuncSetAttribute(conv_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, CV_SMEM1);
+    cudaFuncSetAttribute(conv_tc_kernel<3, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cv_smem(3, F16));
+    cudaFuncSetAttribute(conv_tc_kernel<1, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cv_smem(1, F16));
   }
   if (ksize == 3)
-    conv_tc_kernel<3><<<(unsigned)pl.ctas, CV_THREADS, CV_SMEM3, (cudaStream_t)stream>>>(p);
+    conv_tc_kernel<3, F16><<<(unsigned)pl.ctas, CV_THREADS, cv_smem(3, F16), (cudaStream_t)stream>>>(p);
   else
-    conv_tc_kernel<1><<<(unsigned)pl.ctas, CV_THREADS, CV_SMEM1, (cudaStream_t)stream>>>(p);
-  CUTIE_CHECK_LAUNCH();
-  return 0;
+    conv_tc_kernel<1, F16><<<(unsigned)pl.ctas, CV_THREADS, cv_smem(1, F16), (cudaStream_t)stream>>>(p);
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : ::cutie::set_cuda_error(fn, e);
+}
+
+extern "C" int cutie_conv_tc(const float* x, const int64_t* x_strides, const void* weight_image, const float* bias,
+                             const float* residual, const int64_t* residual_strides, int64_t NB, int64_t Cin, int64_t Cout,
+                             int64_t H_in, int64_t W_in, int ksize, int stride, int relu_in, int relu_out, float* y,
+                             const int64_t* y_strides, int units_per_cta, float* workspace, int32_t* counters, void* stream) {
+  return conv_tc_launch<false>(__func__, x, x_strides, weight_image, bias, residual, residual_strides, NB, Cin, Cout, H_in, W_in,
+                               ksize, stride, relu_in, relu_out, y, y_strides, units_per_cta, workspace, counters, stream);
+}
+
+extern "C" int cutie_conv_tc_f16(const float* x, const int64_t* x_strides, const void* weight_image, const float* bias,
+                                 const float* residual, const int64_t* residual_strides, int64_t NB, int64_t Cin, int64_t Cout,
+                                 int64_t H_in, int64_t W_in, int ksize, int stride, int relu_in, int relu_out, float* y,
+                                 const int64_t* y_strides, int units_per_cta, float* workspace, int32_t* counters, void* stream) {
+  return conv_tc_launch<true>(__func__, x, x_strides, weight_image, bias, residual, residual_strides, NB, Cin, Cout, H_in, W_in,
+                              ksize, stride, relu_in, relu_out, y, y_strides, units_per_cta, workspace, counters, stream);
 }
 
 extern "C" int cutie_debug_conv_tile_shape(int64_t H, int64_t W, int* out3) {

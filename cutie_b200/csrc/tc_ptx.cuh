@@ -1,6 +1,7 @@
 // Inline-PTX helpers for the wgmma / mbarrier / bulk-copy kernels (sm_90a): shared by the affinity filters
 // (affinity_tc.cu, affinity_f16.cu), the object-transformer attention kernels (qt_tc.cu) and the convolutions (conv_tc.cu).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -40,6 +41,11 @@ __device__ __forceinline__ float to_tf32(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
 }
+// two fp32 values as one f16x2 word, each rounded to nearest (overflow -> inf, as Tensor.half()); `a` at the lower address
+__device__ __forceinline__ uint32_t f16x2_rn(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
 
 // ---- warpgroup MMA (sm_90a wgmma): D[64 x N] (+)= A[64 x K] . B[N x K]^T, both operands K-major in shared memory, the
 // fp32 accumulator in the registers of the issuing warpgroup (all 128 threads issue every call).  Fragment: thread
@@ -61,6 +67,16 @@ __device__ __forceinline__ uint64_t desc_sw128_kmajor(uint32_t addr) {
   d |= (uint64_t)1 << 16;                        // leading byte offset: unused for swizzled K-major
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset: 8 rows x 128 B
   d |= (uint64_t)1 << 62;                        // SWIZZLE_128B
+  return d;
+}
+// SWIZZLE_64B K-major: a block is [rows x 64 B] (64 B = 32 f16 along K), 8-row groups 512 B apart (SBO); the 16-byte
+// chunk index (address bits 4-5) is XORed with address bits 7-8; one f16 k16 step = +32 B inside the swizzle atom.
+__device__ __forceinline__ uint64_t desc_sw64_kmajor(uint32_t addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((addr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;                        // leading byte offset: unused for swizzled K-major
+  d |= (uint64_t)(512 >> 4) << 32;               // stride byte offset: 8 rows x 64 B
+  d |= (uint64_t)2 << 62;                        // SWIZZLE_64B
   return d;
 }
 // K-major un-swizzled (interleaved 8 x 16 B core matrices): `lbo` = distance between the 16-byte K chunks, `sbo` = between
@@ -107,6 +123,15 @@ __device__ __forceinline__ void wgmma_f16_n32(float (&d)[16], uint64_t adesc, ui
       "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 

@@ -11,9 +11,12 @@ frame have static shapes and touch no memory-bank pointers, so each is captured 
 The memory read between them (cutie_affinity_topk + cutie_readout_gather) stays eager: its segment pointers move
 whenever the ring advances.  On memory frames the mask encoder + object summarizer (G3) are a third graph; the
 append into the arena stays eager.  Graphs are keyed by every
-shape/flag they depend on and are bypassed (eager path) for multi-bucket / chunked / flip-augmented reads.
+shape/flag they depend on -- including the precision mode (`amp`: the step runs under fp16 autocast, so the model's
+tensor-core convolutions take their FP16-operand form; a capture of one mode is never replayed in the other) -- and are
+bypassed (eager path) for multi-bucket / chunked / flip-augmented reads.
 Enable with `InferenceCore(..., use_cuda_graphs=True)` or `processor.use_cuda_graphs = True`.
 """
+import gc
 from typing import Dict, Tuple
 
 import torch
@@ -33,8 +36,18 @@ class _Captured:
         cur.wait_stream(side)
         self.graph = torch.cuda.CUDAGraph()
         before = K_.LAUNCH_COUNT
-        with torch.cuda.graph(self.graph):
-            self.outputs = fn(*static_inputs)
+        # Python's cyclic collector is paused while capturing: it may run at any allocation, and a dead reference cycle
+        # holding another capture (a discarded InferenceCore: its encoder look-ahead refers back to it) would destroy that
+        # CUDA graph and release its memory pool in the middle of this capture, which invalidates it
+        # (cudaErrorStreamCaptureInvalidated).  torch.cuda.graph collects only with torch.compiler.config.force_cudagraph_gc.
+        gc_on = gc.isenabled()
+        gc.disable()
+        try:
+            with torch.cuda.graph(self.graph):
+                self.outputs = fn(*static_inputs)
+        finally:
+            if gc_on:
+                gc.enable()
         self.kernel_launches = K_.LAUNCH_COUNT - before       # cutie_b200 kernels recorded in this graph
 
     def replay(self):
@@ -51,10 +64,10 @@ class FrameGraphs:
         self._msk: Dict[Tuple, _Captured] = {}
 
     # ---- G1 ------------------------------------------------------------------------------------
-    def encode(self, image: torch.Tensor, slot: int = 0):
+    def encode(self, image: torch.Tensor, slot: int = 0, amp: bool = False):
         """`slot` selects one of several independent captures (own static input and outputs): InferenceCore alternates
         two of them so that the next frame's encoder can run on a side stream while this frame's outputs are in use."""
-        key = (tuple(image.shape), image.device, int(slot))
+        key = (tuple(image.shape), image.device, int(slot), bool(amp))
         cap = self._enc.get(key)
         if cap is None:
             static_img = image.clone()
@@ -68,11 +81,11 @@ class FrameGraphs:
         return cap.replay()
 
     # ---- G2 ------------------------------------------------------------------------------------
-    def segment(self, visual, pix_feat, sensory, last_mask, obj_mem, ms_feat, update_sensory: bool):
+    def segment(self, visual, pix_feat, sensory, last_mask, obj_mem, ms_feat, update_sensory: bool, amp: bool = False):
         """All arguments are tensors; visual/pix_feat/ms_feat may already be graph-static (G1 outputs / the gather
         kernel's fixed output buffer).  Returns (new_sensory or None, logits, prob) in static buffers."""
         key = (tuple(visual.shape), tuple(last_mask.shape), bool(update_sensory), visual.device,
-               tuple(t.data_ptr() for t in (pix_feat, *ms_feat)))
+               tuple(t.data_ptr() for t in (pix_feat, *ms_feat)), bool(amp))
         cap = self._seg.get(key)
         if cap is None:
             st = (visual.clone(), sensory.clone(), last_mask.clone(), obj_mem.clone())
@@ -88,10 +101,10 @@ class FrameGraphs:
         return cap.replay()
 
     # ---- G3 (memory frames) ----------------------------------------------------------------------
-    def encode_mask(self, image, pix_feat, sensory, masks):
+    def encode_mask(self, image, pix_feat, sensory, masks, amp: bool = False):
         """CUTIE.encode_mask (mask encoder + deep sensory update + object summarizer) as one replay.
         Returns (value [B,K,CV,h,w], new_sensory, summaries [B,K,Q,E+1]) in static buffers."""
-        key = (tuple(image.shape), tuple(masks.shape), image.device, pix_feat.data_ptr())
+        key = (tuple(image.shape), tuple(masks.shape), image.device, pix_feat.data_ptr(), bool(amp))
         cap = self._msk.get(key)
         if cap is None:
             st = (image.clone(), sensory.clone(), masks.clone())

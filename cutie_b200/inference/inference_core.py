@@ -6,6 +6,7 @@ Same constructor, `step` signature, return value ([1+K, H, W] probabilities) and
 process_video.py drive it unchanged.  The memory read it calls is the fused-kernel path of
 cutie_b200.inference.memory_manager.
 """
+import contextlib
 import logging
 from typing import Iterable, List, Optional
 
@@ -26,6 +27,12 @@ def _graphable(t: torch.Tensor) -> bool:
     """CUDA graphs (and the encoder look-ahead) need CUDA tensors.  A function so that the CPU suite can drive the graph
     path with stand-in graphs (tests/test_graph_path_cpu.py); the product never changes it."""
     return t.is_cuda
+
+
+def _autocast_state():
+    """(enabled, dtype) of CUDA autocast where step() is called.  A function so that the CPU suite can substitute it
+    (tests/test_amp_policy_cpu.py: without a GPU torch.autocast('cuda') disables itself); the product never changes it."""
+    return torch.is_autocast_enabled('cuda'), torch.get_autocast_dtype('cuda')
 
 
 class _CudaStreamOps:
@@ -76,7 +83,9 @@ class EncoderLookahead:
       * before it, the side stream waits for everything enqueued on the main stream so far -- the end of the previous
         step, whose consumers were the last readers of that slot, and whatever made the announced image valid;
       * the main stream waits for the look-ahead's event before it touches either the outputs (hit) or re-encodes
-        (miss: wrong frame / tensor announced -- the result is discarded, never used)."""
+        (miss: wrong frame / tensor announced -- the result is discarded, never used);
+      * a look-ahead records the precision mode it was encoded under (`mode`: fp32 or amp); a step in the other mode
+        counts it as a miss (the encoder's arithmetic differs between the modes)."""
 
     def __init__(self, encode, ops=None):
         self.encode = encode
@@ -84,7 +93,7 @@ class EncoderLookahead:
         self.slot = 0
         self.pending = None
 
-    def current(self, ti: int, image: torch.Tensor, src_id):
+    def current(self, ti: int, image: torch.Tensor, src_id, mode=None):
         la, self.pending = self.pending, None
         if la is not None:
             self.ops.main_wait_event(la['done'])
@@ -94,12 +103,12 @@ class EncoderLookahead:
             t = la['tensor']
             if (la['ti'] == ti and src_id.data_ptr() == t.data_ptr() and tuple(src_id.shape) == tuple(t.shape)
                     and src_id.stride() == t.stride() and la['version'] == _version_of(src_id)
-                    and la['shape'] == tuple(image.shape)):
+                    and la['shape'] == tuple(image.shape) and la['mode'] == mode):
                 self.slot = la['slot']
                 return la['out'], True
         return self.encode(image, self.slot), False
 
-    def ahead(self, ti: int, next_image: torch.Tensor, prepare):
+    def ahead(self, ti: int, next_image: torch.Tensor, prepare, mode=None):
         dev = next_image.device
         self.ops.side_wait_main(dev)
         self.ops.keep_alive_on_side(next_image)
@@ -109,7 +118,7 @@ class EncoderLookahead:
             out = self.encode(img, slot)
             done = self.ops.record_on_side(dev)
         self.pending = dict(ti=ti + 1, slot=slot, tensor=next_image, version=_version_of(next_image),
-                            shape=tuple(img.shape), out=out, done=done)
+                            shape=tuple(img.shape), out=out, done=done, mode=mode)
 
 
 class InferenceCore:
@@ -142,6 +151,7 @@ class InferenceCore:
         self._graphs = None
         # encoder look-ahead (step(..., next_image=...)): the next frame's image-encoder graph on a side stream
         self._lookahead = None       # EncoderLookahead, created with the graphs
+        self._amp = False            # the current step runs in amp mode (step() under fp16 autocast)
 
     # -- memory control ------------------------------------------------------------------------
     def _reset_clock(self):
@@ -180,7 +190,7 @@ class InferenceCore:
         if graphed:
             with K_._call('region:encode_mask_graph', 0):          # bench.py: device time of the whole replay
                 msk_value, sensory, obj_value = self._graphs.encode_mask(image, pix_feat, self.memory.get_sensory(ids),
-                                                                         prob)
+                                                                         prob, amp=self._amp)
             sensory = sensory.clone()          # outlives this frame; value / summaries are consumed by add_memory below
         else:
             msk_value, sensory, obj_value, _ = self.network.encode_mask(
@@ -212,7 +222,7 @@ class InferenceCore:
             with K_._call('region:segment_graph', 0):
                 last_mask = self.memory._get_mask_by_ids(self.last_mask, ids)     # after delete_objects: live channels only
                 sensory, logits, prob = self._graphs.segment(visual, pix_feat, sens_in, last_mask, obj_mem,
-                                                             tuple(ms_features), update_sensory)
+                                                             tuple(ms_features), update_sensory, amp=self._amp)
             logits, prob = logits.clone(), prob.clone()
             if update_sensory:
                 sensory = sensory.clone()
@@ -254,7 +264,26 @@ class InferenceCore:
         next_image (extension; CUDA-graph path only): the frame the NEXT call will be given.  Its image encoder -- which
         depends on nothing but the image -- is enqueued on a side stream now and overlaps this frame's memory read,
         object transformer and decoder; the next call picks the result up if it is handed the same tensor.  Results
-        are identical with or without it."""
+        are identical with or without it.
+
+        Mixed precision: called under fp16 CUDA autocast (as the reference's scripting_demo.py / eval_vos.py / GUI do),
+        the step runs with autocast switched off -- every PyTorch / cuDNN op stays fp32 -- and the model's convolution
+        fuser in amp mode: the tensor-core convolutions take their FP16-operand form (fuse.ConvEpilogueFuser 'tc16').
+        Inputs and outputs stay fp32.  bf16 autocast raises NotImplementedError."""
+        on, dtype = _autocast_state()
+        self._amp = bool(on)
+        if not on:
+            return self._step(image, mask, objects, idx_mask=idx_mask, end=end, delete_buffer=delete_buffer,
+                              force_permanent=force_permanent, next_image=next_image)
+        if dtype != torch.float16:
+            raise NotImplementedError(f'InferenceCore.step under {dtype} autocast: only float16 autocast is supported')
+        fuser = getattr(self.network, 'conv_epilogues', None)
+        with torch.autocast('cuda', enabled=False), (fuser.amp_mode() if fuser is not None else contextlib.nullcontext()):
+            return self._step(image, mask, objects, idx_mask=idx_mask, end=end, delete_buffer=delete_buffer,
+                              force_permanent=force_permanent, next_image=next_image)
+
+    def _step(self, image: torch.Tensor, mask: Optional[torch.Tensor], objects: Optional[List[int]], *, idx_mask: bool,
+              end: bool, delete_buffer: bool, force_permanent: bool, next_image: Optional[torch.Tensor]) -> torch.Tensor:
         src_id = image               # the caller's tensor itself: a look-ahead hit is decided on its memory + version
         if objects is None and mask is not None:
             assert not idx_mask
@@ -293,7 +322,8 @@ class InferenceCore:
                 self._graphs = FrameGraphs(self.network)
             if self._lookahead is None:
                 self._lookahead = EncoderLookahead(self._encode_graph)
-            (ms_feat, pix_feat, key, shrinkage, selection), _hit = self._lookahead.current(self.curr_ti, image, src_id)
+            (ms_feat, pix_feat, key, shrinkage, selection), _hit = self._lookahead.current(self.curr_ti, image, src_id,
+                                                                                          mode=self._amp)
             if next_image is not None and _graphable(next_image) and not resize_needed:
                 self._encode_ahead(next_image)
         else:
@@ -349,14 +379,14 @@ class InferenceCore:
 
     def _encode_graph(self, image: torch.Tensor, slot: int):
         with K_._call('region:encode_graph', 0):
-            return self._graphs.encode(image, slot)
+            return self._graphs.encode(image, slot, amp=self._amp)
 
     def _encode_ahead(self, next_image: torch.Tensor) -> None:
         """Enqueue G1 (image encoder + key projection) of the next frame on the side stream (EncoderLookahead.ahead);
         this frame's own work is enqueued on the current stream after this call and runs concurrently with it."""
         if self.max_internal_size > 0 and min(next_image.shape[-2:]) > self.max_internal_size:
             return                                    # the internal down-scaling path recomputes on the main stream
-        self._lookahead.ahead(self.curr_ti, next_image, lambda t: pad_divide_by(t, 16)[0].unsqueeze(0))
+        self._lookahead.ahead(self.curr_ti, next_image, lambda t: pad_divide_by(t, 16)[0].unsqueeze(0), mode=self._amp)
 
     def delete_objects(self, objects: List[int]) -> None:
         self.object_manager.delete_objects(objects)

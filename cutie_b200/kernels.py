@@ -450,19 +450,35 @@ def conv_tc_eligible(weight: torch.Tensor, stride=(1, 1), padding=(1, 1), dilati
     return False
 
 
+def conv_weight_image_bytes(cout: int, cin: int, ksize: int, f16: bool = False) -> int:
+    """Bytes of a layer's operand image for cutie_conv_tc (f16=False) or cutie_conv_tc_f16 (f16=True); -1: no such image."""
+    f = lib().cutie_conv_weight_image_f16_bytes if f16 else lib().cutie_conv_weight_image_bytes
+    f.restype = ctypes.c_int64
+    return int(f(_i64(cout), _i64(cin), int(ksize)))
+
+
+def _conv_weight_image(weight: torch.Tensor, f16: bool) -> torch.Tensor:
+    Cout, Cin, k = weight.shape[0], weight.shape[1], weight.shape[2]
+    assert weight.dtype == torch.float32 and weight.shape[2] == weight.shape[3] and k in (1, 3) and Cin % 32 == 0
+    img = torch.empty(conv_weight_image_bytes(Cout, Cin, k, f16) // 4, dtype=torch.float32, device=weight.device)
+    w = weight.detach().contiguous()
+    name = 'conv_weight_image_f16' if f16 else 'conv_weight_image'
+    with _call(name, 1):
+        st = getattr(lib(), 'cutie_' + name)(_ptr(w), _i64(Cout), _i64(Cin), int(k), _ptr(img), _stream())
+    _check(st, 'cutie_' + name)
+    return img
+
+
 def conv_weight_image(weight: torch.Tensor) -> torch.Tensor:
     """The layer's tensor-core operand image (tf32 hi | lo planes per (128-channel tile, 32-channel chunk, tap), swizzled):
     built once per weight version, 2x the weight bytes."""
-    Cout, Cin, k = weight.shape[0], weight.shape[1], weight.shape[2]
-    assert weight.dtype == torch.float32 and weight.shape[2] == weight.shape[3] and k in (1, 3) and Cin % 32 == 0
-    lib().cutie_conv_weight_image_bytes.restype = ctypes.c_int64
-    nbytes = lib().cutie_conv_weight_image_bytes(_i64(Cout), _i64(Cin), int(k))
-    img = torch.empty(nbytes // 4, dtype=torch.float32, device=weight.device)
-    w = weight.detach().contiguous()
-    with _call('conv_weight_image', 1):
-        st = lib().cutie_conv_weight_image(_ptr(w), _i64(Cout), _i64(Cin), int(k), _ptr(img), _stream())
-    _check(st, 'cutie_conv_weight_image')
-    return img
+    return _conv_weight_image(weight, False)
+
+
+def conv_weight_image_f16(weight: torch.Tensor) -> torch.Tensor:
+    """The operand image of conv_tc(..., f16=True): one fp16 plane per (128-channel tile, 32-channel chunk, tap), each
+    weight rounded to nearest, K-major SWIZZLE_64B; half the weight bytes.  (float32 is only the container dtype.)"""
+    return _conv_weight_image(weight, True)
 
 
 def _ncp_strides(t: torch.Tensor):
@@ -479,14 +495,19 @@ def _ncp_strides(t: torch.Tensor):
 def conv_tc(x: torch.Tensor, weight_image: torch.Tensor, bias: Optional[torch.Tensor], cout: int, ksize: int = 3,
             stride: int = 1, residual: Optional[torch.Tensor] = None, relu_in: bool = False,
             relu_out: bool = False, units_per_cta: Optional[int] = None,
-            counters: Optional[torch.Tensor] = None) -> torch.Tensor:
+            counters: Optional[torch.Tensor] = None, f16: bool = False) -> torch.Tensor:
     """act(bias + conv(pre(x)) [+ residual]) on the tensor cores with 3xTF32 splitting (fp32-class accuracy).
     x [N, Cin, H, W] dense NCHW or channels-last (the output takes the same memory format) -> [N, cout, H', W'].
     Layers with fewer output tiles than SMs are spread evenly over the SMs in (tile, input chunk) units (cutie_conv_plan):
     `units_per_cta` overrides the plan's share size (tests); `counters`: the layer's own zeroed int32 tile counters (the
-    kernel leaves them zero), else a fresh zeroed buffer per call."""
+    kernel leaves them zero), else a fresh zeroed buffer per call.
+    f16=True: cutie_conv_tc_f16 -- FP16 operands (pre(x) and the weights rounded to nearest), fp32 accumulation, fp32
+    tensors in and out, as autocast runs a convolution; `weight_image` then comes from conv_weight_image_f16."""
     N, Cin, H, W = x.shape
     assert x.dtype == torch.float32 and ksize in (1, 3)
+    if weight_image.numel() * weight_image.element_size() != conv_weight_image_bytes(cout, Cin, ksize, f16):
+        raise KernelError(f'conv_tc: the weight image does not fit a {ksize}x{ksize} {Cin}->{cout} layer in '
+                          f'{"fp16" if f16 else "3xTF32"} form (build it with conv_weight_image{"_f16" if f16 else ""})')
     cl = x.is_contiguous(memory_format=torch.channels_last) and not x.is_contiguous()
     if not cl:
         x = x.contiguous()
@@ -510,14 +531,20 @@ def conv_tc(x: torch.Tensor, weight_image: torch.Tensor, bias: Optional[torch.Te
     if ws_floats:
         ws = torch.empty(ws_floats, dtype=torch.float32, device=x.device)
         cnt = counters if counters is not None and counters.numel() >= ntile else torch.zeros(ntile, dtype=torch.int32, device=x.device)
-    with _call('conv_tc', 1):
-        st = lib().cutie_conv_tc(_ptr(x), arr(_ncp_strides(x)), _ptr(weight_image),
-                                 _ptr(bias.detach() if bias is not None else None), _ptr(residual),
-                                 arr(zs) if zs is not None else None, _i64(N), _i64(Cin), _i64(cout), _i64(H), _i64(W),
-                                 int(ksize), int(stride), int(bool(relu_in)), int(bool(relu_out)), _ptr(out),
-                                 arr(_ncp_strides(out)), q, _ptr(ws), _ptr(cnt, torch.int32), _stream())
-    _check(st, 'cutie_conv_tc')
+    name = 'conv_tc_f16' if f16 else 'conv_tc'
+    with _call(name, 1):
+        st = getattr(lib(), 'cutie_' + name)(
+            _ptr(x), arr(_ncp_strides(x)), _ptr(weight_image), _ptr(bias.detach() if bias is not None else None),
+            _ptr(residual), arr(zs) if zs is not None else None, _i64(N), _i64(Cin), _i64(cout), _i64(H), _i64(W),
+            int(ksize), int(stride), int(bool(relu_in)), int(bool(relu_out)), _ptr(out), arr(_ncp_strides(out)), q,
+            _ptr(ws), _ptr(cnt, torch.int32), _stream())
+    _check(st, 'cutie_' + name)
     return out
+
+
+def conv_tc_f16(x: torch.Tensor, weight_image: torch.Tensor, bias: Optional[torch.Tensor], cout: int, **kw) -> torch.Tensor:
+    """conv_tc(..., f16=True): the FP16-operand form (weight_image from conv_weight_image_f16)."""
+    return conv_tc(x, weight_image, bias, cout, f16=True, **kw)
 
 
 def area_pool(x: torch.Tensor, f: int) -> torch.Tensor:

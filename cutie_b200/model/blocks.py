@@ -230,6 +230,7 @@ class MultiScaleSensoryUpdater(nn.Module):
         self.g8_conv = ObjConv2d(g_dims[1], mid_dim, 1)
         self.g4_conv = ObjConv2d(g_dims[2], mid_dim, 1)
         self.transform = ObjConv2d(mid_dim + sensory_dim, sensory_dim * 3, 3, padding=1)
+        self.transform.amp_fp32 = True      # fp32 under autocast too, as modules.py:62-64 (a plain attribute: no state_dict key)
 
     def forward(self, g16, g8, g4, h):
         if isinstance(g4, (tuple, list)):
@@ -250,6 +251,7 @@ class DeepSensoryUpdater(nn.Module):
     def __init__(self, f_dim: int, sensory_dim: int):
         super().__init__()
         self.transform = ObjConv2d(f_dim + sensory_dim, sensory_dim * 3, 3, padding=1)
+        self.transform.amp_fp32 = True      # fp32 under autocast too, as modules.py:79-81
 
     def forward(self, g, h):
         return gated_update(h.float(), self.transform(torch.cat([g.float(), h.float()], 2)), self)

@@ -2,6 +2,8 @@
 eval-mode BatchNorm folded into the preceding convolution, ResNet trunks run channels-last so cuDNN's NHWC
 tensor-core kernels need no per-layer NCHW<->NHWC conversion.  Applied AFTER weights are loaded
 (`CUTIE.optimize_for_inference()`); the state_dict layout of an optimised model is no longer the checkpoint's."""
+import contextlib
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F  # noqa: F401
@@ -59,25 +61,40 @@ class ConvEpilogueFuser:
                 kernel -- 3x3 / stride 1 / pad 1 and 1x1 / stride 1 or 2 layers with Cin % 32 == 0 and Cout >= 64, dense
                 NCHW or channels-last (the output keeps the input's memory format): SURVEY.md section 8(f).1-3 --
                 PixelFFN, fuser, key projection, decoder, sensory update and the trunks' bottleneck convolutions
+      'tc16'    cutie_conv_tc_f16: the same kernel with FP16 operands and fp32 accumulation -- what fp16 autocast asks of a
+                convolution; taken instead of 'tc' only in AMP MODE (`amp_mode()`, entered by InferenceCore.step under
+                autocast), except by layers marked `amp_fp32` (the sensory updaters' transforms, which the reference
+                itself runs in autocast(enabled=False))
 
-    DETERMINISTIC: the form is a function of the layer geometry and the epilogue alone -- `RULE`: eligible 3x3 / 1x1 layers take
-    'tc'; of the rest ReLU epilogues take 'cudnn', bias-only and bias+residual epilogues take 'kernel', stems take 'pool' -- (a committed choice, not re-timed per GPU); nothing is timed at run time, so two runs of the
+    DETERMINISTIC: the form is a function of the layer geometry, the epilogue and the mode alone -- `RULE`: eligible 3x3 / 1x1
+    layers take 'tc' ('tc16' in amp mode); of the rest ReLU epilogues take 'cudnn', bias-only and bias+residual epilogues take 'kernel', stems take 'pool' -- (a committed choice, not re-timed per GPU); nothing is timed at run time, so two runs of the
     same video execute the same arithmetic.  CPU tensors (the oracle harness borrowing these modules) always take 'aten'.
 
     `cudnn_convolution_relu` hands the *uninitialised* output to cuDNN as the residual operand with alpha = 0;
     0 x (stale NaN bits) is NaN, so the no-residual case passes a persistent zero tensor of the output shape
     instead (read once per call, ~100 MB per 480p frame over all layers: 15 us of HBM time).
     """
-    FORMS = ('aten', 'cudnn', 'kernel', 'tc')
+    FORMS = ('aten', 'cudnn', 'kernel', 'tc', 'tc16')
     RULE = {'conv': 'tc', 'relu': 'cudnn', 'linear': 'kernel', 'stem': 'pool'}
 
     def __init__(self, enabled: bool = True, rule=None):
         self.enabled = enabled
         self.rule = dict(self.RULE if rule is None else rule)
+        self.amp = False             # amp mode: eligible 'tc' layers take 'tc16' (amp_mode())
         self.counts = {}             # form -> number of distinct (layer, geometry, epilogue) triples routed to it
         self._seen = set()
         self._zeros = {}
-        self._images = {}            # id(conv) -> (weight identity, operand image) of the 'tc' form
+        self._images = {}            # id(conv) -> (weight identity, operand image, counters) of the 'tc' form
+        self._images16 = {}          # ... of the 'tc16' form
+
+    @contextlib.contextmanager
+    def amp_mode(self, on: bool = True):
+        """Within the block eligible layers take the FP16-operand form 'tc16' (layers marked `amp_fp32` keep 'tc')."""
+        prev, self.amp = self.amp, bool(on)
+        try:
+            yield self
+        finally:
+            self.amp = prev
 
     # -- the forms ------------------------------------------------------------------------------------
     @staticmethod
@@ -123,22 +140,27 @@ class ConvEpilogueFuser:
         from cutie_b200 import kernels as K_
         return K_.bias_act_(self._conv(conv, x, False), conv.bias, z, relu)
 
-    def tensor_core(self, conv: nn.Conv2d, x: torch.Tensor, z=None, relu: bool = True, relu_in: bool = False) -> torch.Tensor:
-        """The 'tc' form.  The operand image is rebuilt whenever the weight tensor is replaced or written."""
+    def tensor_core(self, conv: nn.Conv2d, x: torch.Tensor, z=None, relu: bool = True, relu_in: bool = False,
+                    f16: bool = False) -> torch.Tensor:
+        """The 'tc' form ('tc16' with f16=True).  The operand image is rebuilt whenever the weight tensor is replaced or
+        written."""
         from cutie_b200 import kernels as K_
         w = conv.weight
         try:
             ident = (w.data_ptr(), w._version)
         except RuntimeError:                       # inference tensors carry no version counter
             ident = (w.data_ptr(), None)
-        hit = self._images.get(id(conv))
+        images = self._images16 if f16 else self._images
+        hit = images.get(id(conv))
         if hit is None or hit[0] != ident:
             # the layer's operand image and its own shared-tile counters (zero between launches; one layer never runs
             # twice at the same time, different layers may -- encoder look-ahead -- so counters are never shared)
-            hit = (ident, K_.conv_weight_image(w), torch.zeros(8192, dtype=torch.int32, device=w.device))
-            self._images[id(conv)] = hit
-        return K_.conv_tc(x, hit[1], conv.bias, conv.out_channels, ksize=conv.kernel_size[0], stride=conv.stride[0],
-                          residual=z, relu_in=relu_in, relu_out=relu, counters=hit[2])
+            img = K_.conv_weight_image_f16(w) if f16 else K_.conv_weight_image(w)
+            hit = (ident, img, torch.zeros(8192, dtype=torch.int32, device=w.device))
+            images[id(conv)] = hit
+        return (K_.conv_tc_f16 if f16 else K_.conv_tc)(x, hit[1], conv.bias, conv.out_channels, ksize=conv.kernel_size[0],
+                                                       stride=conv.stride[0], residual=z, relu_in=relu_in, relu_out=relu,
+                                                       counters=hit[2])
 
     def _tc_eligible(self, conv: nn.Conv2d, x: torch.Tensor, z) -> bool:
         from cutie_b200 import kernels as K_
@@ -148,6 +170,8 @@ class ConvEpilogueFuser:
     def run(self, form: str, conv: nn.Conv2d, x: torch.Tensor, z=None, relu: bool = True, relu_in: bool = False) -> torch.Tensor:
         if form == 'tc':
             return self.tensor_core(conv, x, z, relu, relu_in)
+        if form == 'tc16':
+            return self.tensor_core(conv, x, z, relu, relu_in, f16=True)
         if relu_in:
             x = F.relu(x)
         if form == 'cudnn':
@@ -170,7 +194,7 @@ class ConvEpilogueFuser:
         if not self._eligible(conv, x):
             return self.unfused(conv, x, z, relu, relu_in)
         if self._tc_eligible(conv, x, z):
-            form = 'tc'
+            form = 'tc16' if self.amp and not getattr(conv, 'amp_fp32', False) else 'tc'
         else:
             form = self.rule['relu'] if relu else self.rule['linear']
         self._note(form, conv, x, z, relu)
@@ -195,6 +219,7 @@ class ConvEpilogueFuser:
         return new
 
     def report(self) -> dict:
+        """`layers`: form -> distinct (layer, geometry, epilogue) triples routed to it so far, amp steps' 'tc16' included."""
         return {'enabled': self.enabled, 'rule': dict(self.rule), 'layers': dict(self.counts)}
 
 

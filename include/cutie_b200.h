@@ -15,7 +15,9 @@
  *   - all work is enqueued on `stream` (a cudaStream_t passed as void*); nothing synchronises;
  *   - return 0 on success, <0 on invalid argument (-1) or launch failure (-2); never throws;
  *     cutie_b200_last_error() returns a thread-local message for the last failure;
- *   - all floating point is fp32 (the reference runs this path with amp=False, eval_config.yaml:13);
+ *   - all floating-point data is fp32 (the reference runs this path with amp=False, eval_config.yaml:13); the one
+ *     reduced-precision form, cutie_conv_tc_f16 (the reference's drivers under autocast), also takes and returns fp32
+ *     tensors: only its operand image and the operands inside the kernel are fp16;
  *   - "token-major" = [B, n, C] with the channel axis contiguous (one memory token per row);
  *     "channel-major" = [B, C, n] as PyTorch convolutions emit feature maps.
  */
@@ -184,7 +186,21 @@ int cutie_conv_tc(const float* x, const int64_t* x_strides, const void* weight_i
                   const float* residual, const int64_t* residual_strides, int64_t NB, int64_t Cin, int64_t Cout,
                   int64_t H_in, int64_t W_in, int ksize, int stride, int relu_in, int relu_out, float* y,
                   const int64_t* y_strides, int units_per_cta, float* workspace, int32_t* counters, void* stream);
-/* Launch plan of cutie_conv_tc: out6 = {output tiles T (images x 128-channel tiles x spatial tiles), MMA N, input chunks C per
+/* The same convolution with FP16 operands: what the reference's drivers ask for when they run step() under CUDA autocast
+ * (scripting_demo.py:13 `@torch.cuda.amp.autocast()`, cutie/eval_vos.py:112 `autocast(enabled=use_amp)`), where
+ * PyTorch runs these layers as cuDNN fp16 convolutions.  Same arguments, geometry, plan (cutie_conv_plan: tiles,
+ * workspace, counters) and epilogues as cutie_conv_tc, and x / bias / residual / y stay fp32: pre(x) and the weights are
+ * rounded to fp16 (round to nearest, overflow -> inf), products are exact and accumulate in fp32 (one
+ * wgmma.m64n128k16.f32.f16.f16 per 16 input channels and tap).  `weight_image` comes from cutie_conv_weight_image_f16:
+ * cutie_conv_weight_image_f16_bytes(Cout, Cin, k) bytes, one fp16 [128 x 32] plane per (128-channel tile, 32-channel
+ * chunk, tap) in K-major SWIZZLE_64B order (8 KB per MMA step, a quarter of the 3xTF32 image). */
+int64_t cutie_conv_weight_image_f16_bytes(int64_t Cout, int64_t Cin, int ksize);
+int cutie_conv_weight_image_f16(const float* weight, int64_t Cout, int64_t Cin, int ksize, void* image, void* stream);
+int cutie_conv_tc_f16(const float* x, const int64_t* x_strides, const void* weight_image, const float* bias,
+                      const float* residual, const int64_t* residual_strides, int64_t NB, int64_t Cin, int64_t Cout,
+                      int64_t H_in, int64_t W_in, int ksize, int stride, int relu_in, int relu_out, float* y,
+                      const int64_t* y_strides, int units_per_cta, float* workspace, int32_t* counters, void* stream);
+/* Launch plan of cutie_conv_tc and cutie_conv_tc_f16: out6 = {output tiles T (images x 128-channel tiles x spatial tiles), MMA N, input chunks C per
  * tile, (tile, chunk) units per CTA q, CTAs, workspace floats}.  CTA i owns units [i q, (i + 1) q) of the T x C space (any
  * q <= C is valid: a share spans at most two tiles): layers with at least as many tiles as SMs run one whole tile per CTA
  * (q = C, no workspace); smaller layers split every tile uniformly over input-channel ranges (q = C / s, the largest s <= 8
