@@ -13,7 +13,8 @@
 //
 //   * A (weights) comes from a precomputed OPERAND IMAGE (cutie_conv_weight_image, built once per layer): for every
 //     (128-channel output tile, 32-channel input chunk, tap) the [128 x 32] tf32 hi and lo planes in K-major
-//     SWIZZLE_128B order, 32 KB, fetched by ONE cp.async.bulk per step through a 3-stage mbarrier ring.
+//     SWIZZLE_128B order, 32 KB, fetched through a 3-stage mbarrier ring.  Each MMA warpgroup reads only its own 64 rows
+//     of a stage, so each refills its own half (a ring per warpgroup): one elected thread bulk-copies its hi and lo rows.
 //   * B (activations), 3x3: the CTA's spatial tile is TH x TW output pixels; its input window with the 1-pixel halo is laid
 //     out in shared memory ONCE per 32-channel chunk as rows of a local zero-padded grid -- row r = ly * (TW + 2) + lx + 1
 //     holds the 32 channels of input pixel (ty0 + ly - 1, tx0 + lx - 1) as 128 bytes, K-major SWIZZLE_128B, hi and lo
@@ -27,7 +28,7 @@
 //     one after the other: tap (dy, dx) reads plane (dy != 1, dx != 1) at (u, v) = (oy - [dy == 0], ox - [dx == 0]) -- again
 //     a constant row shift per tap.  The tile holds 4x the input per output, so N is ~32-48 positions per CTA.
 //     1x1: a tile is 128 consecutive output pixels of the flattened image (stride 2: of the sub-sampled one), no halo; four
-//     activation stages of 32 KB instead of two of 62 KB, filled by two producer groups that take the chunks in turn.
+//     activation stages of 32 KB instead of two of 62 KB, each producer thread keeping two chunks of loads in flight.
 //   * Layout-agnostic: X, Y and Z are addressed through (image, channel, pixel) strides -- dense NCHW (what the transformer
 //     kernels emit) and channels-last (what the cuDNN trunks run in) both work without a re-layout; channels-last is the
 //     natural one (a producer thread reads its 32 channels as 8 x 16 bytes, an epilogue warp stores 32 consecutive channels).
@@ -48,9 +49,11 @@
 //     ((chunk ^ (row >> 1)) & 3 with row counted from the base) is the address-based one and a start shifted by r rows of
 //     64 bytes reads rows r.. of it.  The fresh-accumulator-per-step promotion is kept (DESIGN.md section 3.7).
 //
-// Warp roles (544 threads): warps 0-7 two MMA + epilogue warpgroups (output channels 0-63 / 64-127 of the tile), warps
-// 8-15 activation producers (global fp32 -> hi/lo -> swizzled smem, next chunk's loads in flight during the current
-// chunk's MMAs), warp 16 weight loader (one thread).
+// Warp roles (384 threads = three warpgroups): warps 0-7 two MMA + epilogue warpgroups (output channels 0-63 / 64-127 of
+// the tile; thread 0 of each also refills its weight ring), warps 8-11 activation producers (global fp32 -> hi/lo ->
+// swizzled smem, next chunk's loads in flight during the current chunk's MMAs).  Three warpgroups put three warps on each
+// SM sub-partition, so the per-thread register budget (168) holds both accumulators without spilling; a 17-warp block
+// (5 warps on one sub-partition) capped it at 96 and spilled the promotion's total to local memory on every step.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 
@@ -61,8 +64,9 @@ namespace {
 constexpr int CV_M = 128;                         // output channels per CTA
 constexpr int CV_KC = 32;                         // input channels per chunk
 constexpr int CV_A_STAGES = 3;
-constexpr int CV_THREADS = 544;
-constexpr int CV_PROD = 256;
+constexpr int CV_THREADS = 384;
+constexpr int CV_WARPS = CV_THREADS / 32;
+constexpr int CV_PROD = 128;
 constexpr int CV3_ROWS = 248;                     // 3x3: activation tile rows per stage (31 x 8: planes stay 1024-byte aligned)
 constexpr int CV1_ROWS = 128;                     // 1x1
 constexpr int CV_STAGING = 65 * 1024;             // the finished tile staged as fp32 [128][N | 1 <= 129] (66048 B), 1 KB aligned
@@ -78,7 +82,7 @@ __host__ __device__ constexpr int cv_x_bytes(int ks, bool f16) {
 }
 
 struct ConvTail {
-  unsigned long long a_full[CV_A_STAGES], a_empty[CV_A_STAGES], x_full[4], x_empty[4];
+  unsigned long long a_full[2][CV_A_STAGES], a_empty[2][CV_A_STAGES], x_full[4], x_empty[4];   // a_*: per MMA warpgroup
   int last[2];
 };
 // 3xTF32: 126976 (3x3) | 131072 (1x1) activation bytes + 3 x 32 KB weight stages; FP16: 66560 + 3 x 8 KB
@@ -127,9 +131,9 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
   constexpr int XST = KS == 3 ? 2 : 4;                       // activation stages
   constexpr int A_BYTES = cv_a_bytes(F16);
   constexpr int TAPS = KS * KS;
-  constexpr int HALVES = KS == 3 ? 1 : 2;                    // producer threads per tile row (1x1: 16 channels each)
-  constexpr int CPT = CV_KC / HALVES;                        // channels per producer thread and chunk
+  constexpr int RPT = KS == 3 ? 2 : 1;                       // tile rows per producer thread (3x3: r and r + 128)
   constexpr int DEPTH = KS == 3 ? 1 : 2;                     // chunks of global loads in flight per producer thread
+  constexpr int A_HALF = 64 * ROWB;                          // one warpgroup's rows of one weight plane
   extern __shared__ __align__(1024) unsigned char smem[];
   unsigned char* Xs = smem;
   unsigned char* As = smem + cv_x_bytes(KS, F16);
@@ -165,7 +169,8 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
   const bool direct = nparts == 1 && part0.nslots == 1;
 
   if (tid == 0) {
-    for (int s = 0; s < CV_A_STAGES; ++s) { mbar_init(smem_u32(&T.a_full[s]), 1); mbar_init(smem_u32(&T.a_empty[s]), 256); }
+    for (int G = 0; G < 2; ++G)
+      for (int s = 0; s < CV_A_STAGES; ++s) { mbar_init(smem_u32(&T.a_full[G][s]), 1); mbar_init(smem_u32(&T.a_empty[G][s]), 128); }
     for (int s = 0; s < XST; ++s) { mbar_init(smem_u32(&T.x_full[s]), CV_PROD); mbar_init(smem_u32(&T.x_empty[s]), 256); }
     T.last[0] = T.last[1] = 0;
     mbar_init_fence();
@@ -176,17 +181,17 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
   // by the epilogue AND producer warps, a warp per (channel, tile row): 128-byte coalesced stores, residual read likewise.
   // Channels-last outputs are coalesced either way, but four epilogue warps with 32 accesses in flight each cannot keep
   // HBM busy on the wide, shallow layers (a bottleneck's closing 1x1 + residual ran at 0.5 TB/s): the same staging
-  // ([position][channel]) lets all sixteen warps move 16 bytes per lane, residual included.
+  // ([position][channel]) lets all twelve warps move 16 bytes per lane, residual included.
   const bool staged_nchw = p.ys_p == 1 && (p.z == nullptr || p.zs_p == 1);
   const bool staged = staged_nchw || p.cl_vec;
   const int LD = p.N | 1;                                     // odd row pitch: conflict-free both ways
-  auto store_staged_rows = [&](const ConvPart& P, int sw) {  // sw = 0..15
+  auto store_staged_rows = [&](const ConvPart& P, int sw) {  // sw = warp, 0..CV_WARPS - 1
     const float* stage = reinterpret_cast<const float*>(smem);
     if (!staged_nchw) {                                      // channels-last: a warp per position, 4 channels per lane
       const int co4 = P.cot * CV_M + 4 * lane;
       if (co4 >= p.Cout) return;
       const float4 b4 = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + co4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int j = sw; j < p.N; j += 16) {
+      for (int j = sw; j < p.N; j += CV_WARPS) {
         long long pix;
         bool ok;
         if (KS == 3) {
@@ -211,7 +216,7 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
       return;
     }
     const int nseg = CV_M * (KS == 3 ? p.TH : 1);
-    for (int seg = sw; seg < nseg; seg += 16) {
+    for (int seg = sw; seg < nseg; seg += CV_WARPS) {
       const int col = KS == 3 ? seg / p.TH : seg, ty = KS == 3 ? seg - col * p.TH : 0;
       const int co = P.cot * CV_M + col;
       if (co >= p.Cout) continue;
@@ -240,7 +245,7 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
     }
   };
 
-  // Shared tiles: the CTA that arrived last adds the tile's shares IN SLOT ORDER -- all sixteen warps, 16 bytes per lane
+  // Shared tiles: the CTA that arrived last adds the tile's shares IN SLOT ORDER -- all twelve warps, 16 bytes per lane
   // (four warps with scalar loads left this on the critical path at ~15 us per tile).  Channels-last outputs are finished
   // right here; dense-NCHW ones go through the staging buffer (transposed) and store_staged_rows.
   auto reduce_shares = [&](const ConvPart& P, int sw, bool to_stage) {
@@ -249,7 +254,7 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
     float* stage = reinterpret_cast<float*>(smem);
     const bool co_ok = co4 < p.Cout;
     const float4 b4 = (!to_stage && p.bias && co_ok) ? __ldg(reinterpret_cast<const float4*>(p.bias + co4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int j = sw; j < p.N; j += 16) {
+    for (int j = sw; j < p.N; j += CV_WARPS) {
       long long pix = 0;
       bool ok = true;
       if (!to_stage) {
@@ -284,55 +289,64 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
     }
   };
 
-  if (warp >= 8 && warp < 16) {
-    // ============ activation producers: thread == tile row (1x1: half a row, 16 channels) ============
+  if (warp >= 8) {
+    // ===== activation producers: thread == tile rows pt and pt + 128 (3x3) | row pt (1x1), all 32 channels of each =====
     const int pt = tid - 256;
-    const int r = pt / HALVES, half = pt % HALVES;
-    const bool row_live = r < XROWS;
     int xc = 0;                                              // chunks produced so far (stage ring position)
     for (int pi = 0; pi < nparts; ++pi) {
       const ConvPart& P = pi ? part1 : part0;
       const int chunks = P.c1 - P.c0;
-      bool valid = false;
-      long long poff = 0;
-      if (KS == 3) {
-        if (p.stride == 1) {
-          const int rows_used = p.N + 2 * TWp + 2;
-          if (r >= 1 && r < rows_used) {
-            const int q = r - 1, ly = q / TWp, lx = q - ly * TWp;
-            const int gy = P.ty0 + ly - 1, gx = P.tx0 + lx - 1;
-            valid = ly < p.TH + 2 && gy >= 0 && gy < p.Hi && gx >= 0 && gx < p.Wi;
+      bool valid[RPT];
+      const float* xb[RPT];
+#pragma unroll
+      for (int h = 0; h < RPT; ++h) {
+        const int r = pt + CV_PROD * h;
+        bool ok = false;
+        long long poff = 0;
+        if (KS == 3) {
+          if (p.stride == 1) {
+            const int rows_used = p.N + 2 * TWp + 2;
+            if (r >= 1 && r < rows_used) {
+              const int q = r - 1, ly = q / TWp, lx = q - ly * TWp;
+              const int gy = P.ty0 + ly - 1, gx = P.tx0 + lx - 1;
+              ok = ly < p.TH + 2 && gy >= 0 && gy < p.Hi && gx >= 0 && gx < p.Wi;
+              poff = (long long)gy * p.Wi + gx;
+            }
+          } else {
+            // stride 2: four parity planes P[a][b](u, v) = in(2u + a, 2v + b), each a local (TH + 1) x (TW + 1) grid whose
+            // first row / column is u = ty0 - 1 / v = tx0 - 1; tap (dy, dx) reads plane (dy != 1, dx != 1) shifted by
+            // (dy == 0, dx == 0)
+            const int pl = r / p.plane_rows, q = r - pl * p.plane_rows;
+            const int lu = q / TWp, lv = q - lu * TWp;
+            const int gy = 2 * (P.ty0 - 1 + lu) + (pl >> 1), gx = 2 * (P.tx0 - 1 + lv) + (pl & 1);
+            ok = pl < 4 && lu <= p.TH && gy >= 0 && gy < p.Hi && gx >= 0 && gx < p.Wi;
             poff = (long long)gy * p.Wi + gx;
           }
         } else {
-          // stride 2: four parity planes P[a][b](u, v) = in(2u + a, 2v + b), each a local (TH + 1) x (TW + 1) grid whose first
-          // row / column is u = ty0 - 1 / v = tx0 - 1; tap (dy, dx) reads plane (dy != 1, dx != 1) shifted by (dy == 0, dx == 0)
-          const int pl = r / p.plane_rows, q = r - pl * p.plane_rows;
-          const int lu = q / TWp, lv = q - lu * TWp;
-          const int gy = 2 * (P.ty0 - 1 + lu) + (pl >> 1), gx = 2 * (P.tx0 - 1 + lv) + (pl & 1);
-          valid = pl < 4 && lu <= p.TH && gy >= 0 && gy < p.Hi && gx >= 0 && gx < p.Wi;
-          poff = (long long)gy * p.Wi + gx;
-        }
-      } else {
-        const long long op = P.pix0 + r;
-        if (r < p.N && op < HW) {
-          const int oy = (int)(op / p.W), ox = (int)(op - (long long)oy * p.W);
-          valid = true;
-          poff = (long long)(oy * p.stride) * p.Wi + ox * p.stride;
-        }
-      }
-      const float* xb = p.x + (long long)P.nb * p.xs_n + poff * p.xs_p + (long long)(P.c0 * CV_KC + half * CPT) * p.xs_c;
-      float v[DEPTH][CPT];
-      auto load = [&](int c, float (&dst)[CPT]) {
-        if (p.x_vec) {                                         // channels-last: consecutive floats
-#pragma unroll
-          for (int k4 = 0; k4 < CPT / 4; ++k4) {
-            const float4 f = valid ? __ldg(reinterpret_cast<const float4*>(xb + c * CV_KC + 4 * k4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            dst[4 * k4] = f.x; dst[4 * k4 + 1] = f.y; dst[4 * k4 + 2] = f.z; dst[4 * k4 + 3] = f.w;
+          const long long op = P.pix0 + r;
+          if (r < p.N && op < HW) {
+            const int oy = (int)(op / p.W), ox = (int)(op - (long long)oy * p.W);
+            ok = true;
+            poff = (long long)(oy * p.stride) * p.Wi + ox * p.stride;
           }
-        } else {
+        }
+        valid[h] = ok;
+        xb[h] = p.x + (long long)P.nb * p.xs_n + poff * p.xs_p + (long long)(P.c0 * CV_KC) * p.xs_c;
+      }
+      float v[DEPTH][RPT][CV_KC];
+      auto load = [&](int c, float (&dst)[RPT][CV_KC]) {     // every row's loads of chunk c issued before any is used
 #pragma unroll
-          for (int i = 0; i < CPT; ++i) dst[i] = valid ? __ldg(xb + (long long)(c * CV_KC + i) * p.xs_c) : 0.f;
+        for (int h = 0; h < RPT; ++h) {
+          if (p.x_vec) {                                       // channels-last: consecutive floats
+#pragma unroll
+            for (int k4 = 0; k4 < CV_KC / 4; ++k4) {
+              const float4 f = valid[h] ? __ldg(reinterpret_cast<const float4*>(xb[h] + c * CV_KC + 4 * k4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+              dst[h][4 * k4] = f.x; dst[h][4 * k4 + 1] = f.y; dst[h][4 * k4 + 2] = f.z; dst[h][4 * k4 + 3] = f.w;
+            }
+          } else {
+#pragma unroll
+            for (int i = 0; i < CV_KC; ++i) dst[h][i] = valid[h] ? __ldg(xb[h] + (long long)(c * CV_KC + i) * p.xs_c) : 0.f;
+          }
         }
       };
 #pragma unroll
@@ -346,29 +360,35 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
           if (c < chunks) {
             const int s = xc % XST;
             mbar_wait(smem_u32(&T.x_empty[s]), ((xc / XST) & 1) ^ 1);
-            if (F16 && row_live) {
-              unsigned char* row = Xs + s * XSTAGE + r * ROWB;
 #pragma unroll
-              for (int k8 = 0; k8 < CPT / 8; ++k8) {
-                float f[8];
+            for (int rh = 0; rh < RPT; ++rh) {
+              const int r = pt + CV_PROD * rh;
+              if (r >= XROWS) continue;
+              const float* src = v[d][rh];
+              if (F16) {
+                unsigned char* row = Xs + s * XSTAGE + r * ROWB;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) f[i] = p.relu_in ? fmaxf(v[d][8 * k8 + i], 0.f) : v[d][8 * k8 + i];
-                const int off = ((half * (CPT / 8) + k8) ^ ((r >> 1) & 3)) << 4;
-                *reinterpret_cast<uint4*>(row + off) =
-                    make_uint4(f16x2_rn(f[0], f[1]), f16x2_rn(f[2], f[3]), f16x2_rn(f[4], f[5]), f16x2_rn(f[6], f[7]));
-              }
-            } else if (row_live) {
-              unsigned char* hi = Xs + s * XSTAGE + r * 128;
-              unsigned char* lo = hi + XPLANE;
+                for (int k8 = 0; k8 < CV_KC / 8; ++k8) {
+                  float f[8];
 #pragma unroll
-              for (int k4 = 0; k4 < CPT / 4; ++k4) {
-                float4 f = make_float4(v[d][4 * k4], v[d][4 * k4 + 1], v[d][4 * k4 + 2], v[d][4 * k4 + 3]);
-                if (p.relu_in) f = make_float4(fmaxf(f.x, 0.f), fmaxf(f.y, 0.f), fmaxf(f.z, 0.f), fmaxf(f.w, 0.f));
-                const float4 h = make_float4(to_tf32(f.x), to_tf32(f.y), to_tf32(f.z), to_tf32(f.w));
-                const float4 l = make_float4(to_tf32(f.x - h.x), to_tf32(f.y - h.y), to_tf32(f.z - h.z), to_tf32(f.w - h.w));
-                const int off = ((half * (CPT / 4) + k4) ^ (r & 7)) << 4;
-                *reinterpret_cast<float4*>(hi + off) = h;
-                *reinterpret_cast<float4*>(lo + off) = l;
+                  for (int i = 0; i < 8; ++i) f[i] = p.relu_in ? fmaxf(src[8 * k8 + i], 0.f) : src[8 * k8 + i];
+                  const int off = (k8 ^ ((r >> 1) & 3)) << 4;
+                  *reinterpret_cast<uint4*>(row + off) =
+                      make_uint4(f16x2_rn(f[0], f[1]), f16x2_rn(f[2], f[3]), f16x2_rn(f[4], f[5]), f16x2_rn(f[6], f[7]));
+                }
+              } else {
+                unsigned char* hi = Xs + s * XSTAGE + r * 128;
+                unsigned char* lo = hi + XPLANE;
+#pragma unroll
+                for (int k4 = 0; k4 < CV_KC / 4; ++k4) {
+                  float4 f = make_float4(src[4 * k4], src[4 * k4 + 1], src[4 * k4 + 2], src[4 * k4 + 3]);
+                  if (p.relu_in) f = make_float4(fmaxf(f.x, 0.f), fmaxf(f.y, 0.f), fmaxf(f.z, 0.f), fmaxf(f.w, 0.f));
+                  const float4 h = make_float4(to_tf32(f.x), to_tf32(f.y), to_tf32(f.z), to_tf32(f.w));
+                  const float4 l = make_float4(to_tf32(f.x - h.x), to_tf32(f.y - h.y), to_tf32(f.z - h.z), to_tf32(f.w - h.w));
+                  const int off = (k4 ^ (r & 7)) << 4;
+                  *reinterpret_cast<float4*>(hi + off) = h;
+                  *reinterpret_cast<float4*>(lo + off) = l;
+                }
               }
             }
             fence_proxy_async();
@@ -379,27 +399,28 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
         }
       }
     }
-  } else if (warp == 16) {
-    // ================================== weight loader ==================================
-    if (lane == 0) {
-      int i = 0;
-      for (int pi = 0; pi < nparts; ++pi) {
-        const ConvPart& P = pi ? part1 : part0;
-        const unsigned char* wsrc = p.wimg + ((size_t)P.cot * C + P.c0) * TAPS * A_BYTES;
-        const int steps = (P.c1 - P.c0) * TAPS;
-        for (int k = 0; k < steps; ++k, ++i) {
-          const int s = i % CV_A_STAGES;
-          mbar_wait(smem_u32(&T.a_empty[s]), ((i / CV_A_STAGES) & 1) ^ 1);
-          mbar_arrive_expect_tx(smem_u32(&T.a_full[s]), A_BYTES);
-          bulk_g2s(smem_u32(As + s * A_BYTES), wsrc + (size_t)k * A_BYTES, A_BYTES, smem_u32(&T.a_full[s]));
-        }
-      }
-    }
   } else {
     // ======================= MMA + epilogue: warpgroup G == output channels 64 G .. 64 G + 63 =======================
     const int G = warp >> 2, g = lane >> 2, t4 = lane & 3;
     const int cbase = 64 * G + 16 * (warp & 3) + g;          // fragment element 4 j + 2 h + e: channel cbase + 8 h,
     int i = 0, xc = 0;                                       // position 8 j + 2 t4 + e
+    // The warpgroup's weight ring: rows 64 G .. 64 G + 63 of every plane of weight step j (both parts' steps in turn) go
+    // to the same rows of stage j % CV_A_STAGES, copied by the warpgroup's thread 0 once its 128 threads have freed them.
+    const int steps0 = (part0.c1 - part0.c0) * TAPS;
+    const int nsteps = steps0 + (nparts == 2 ? (part1.c1 - part1.c0) * TAPS : 0);
+    const bool issuer = (tid & 127) == 0;
+    // first image step of each part, as scalars: the tap loop then reads no ConvPart (those live in local memory)
+    const int wstep0 = (part0.cot * C + part0.c0) * TAPS, wstep1 = (part1.cot * C + part1.c0) * TAPS - steps0;
+    auto issue_weights = [&](int j) {
+      const unsigned char* src = p.wimg + (size_t)((j < steps0 ? wstep0 : wstep1) + j) * A_BYTES + G * A_HALF;
+      const int s = j % CV_A_STAGES;
+      const uint32_t dst = smem_u32(As + s * A_BYTES) + G * A_HALF, bar = smem_u32(&T.a_full[G][s]);
+      mbar_arrive_expect_tx(bar, cv_planes(F16) * A_HALF);
+#pragma unroll
+      for (int pl = 0; pl < cv_planes(F16); ++pl) bulk_g2s(dst + pl * CV_M * ROWB, src + pl * CV_M * ROWB, A_HALF, bar);
+    };
+    if (issuer)
+      for (int j = 0; j < CV_A_STAGES && j < nsteps; ++j) issue_weights(j);
     for (int pi = 0; pi < nparts; ++pi) {
       const ConvPart& P = pi ? part1 : part0;
       const int chunks = P.c1 - P.c0;
@@ -414,7 +435,7 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
 #pragma unroll 1
         for (int t = 0; t < TAPS; ++t, ++i) {
           const int s = i % CV_A_STAGES;
-          mbar_wait(smem_u32(&T.a_full[s]), (i / CV_A_STAGES) & 1);
+          mbar_wait(smem_u32(&T.a_full[G][s]), (i / CV_A_STAGES) & 1);
           const uint32_t a_hi = smem_u32(As + s * A_BYTES) + G * 64 * ROWB, a_lo = a_hi + CV_M * 128;
           const uint32_t shift = KS == 3 ? (uint32_t)p.shift[t] * ROWB : 0u;
           wg_fence();
@@ -436,7 +457,11 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
           wg_commit();
           wg_wait0();
           wg_fence_acc(d);
-          mbar_arrive(smem_u32(&T.a_empty[s]));
+          mbar_arrive(smem_u32(&T.a_empty[G][s]));
+          if (issuer && i + CV_A_STAGES < nsteps) {
+            mbar_wait(smem_u32(&T.a_empty[G][s]), (i / CV_A_STAGES) & 1);
+            issue_weights(i + CV_A_STAGES);
+          }
 #pragma unroll
           for (int k = 0; k < 64; ++k) tot[k] += d[k];
         }
@@ -495,55 +520,53 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_tc_kernel(const ConvTcPara
       }
     }
   }
-  // ================================== finish: the sixteen MMA + producer warps ==================================
-  if (warp < 16) {
-    for (int pi = 0; pi < nparts; ++pi) {
-      const ConvPart& P = pi ? part1 : part0;
-      asm volatile("bar.sync 2, 512;" ::: "memory");          // direct: the tile is staged; shares: who stores it is known
-      const bool fin = T.last[pi] != 0;
-      if (!direct && fin) {
-        __threadfence();
-        if (staged_nchw) {
-          reduce_shares(P, warp, true);
-        } else if (p.cl_vec) {
-          reduce_shares(P, warp, false);
-        } else if (warp < 4) {                               // odd layouts: thread == channel, element-wise
-          const float* wst = p.ws + (P.tile_lin * p.maxslots) * (long long)(p.N * CV_M);
-          const int co = P.cot * CV_M + tid;
-          const float b = (p.bias && co < p.Cout) ? __ldg(p.bias + co) : 0.f;
-          float* yb = p.y + (long long)P.nb * p.ys_n + (long long)co * p.ys_c;
-          const float* zb = p.z ? p.z + (long long)P.nb * p.zs_n + (long long)co * p.zs_c : nullptr;
-          for (int j = 0; j < p.N; ++j) {
-            bool ok;
-            long long pix;
-            if (KS == 3) {
-              const int ty = j / TWp, lx = j - ty * TWp;
-              const int gy = P.ty0 + ty, gx = P.tx0 + lx - p.xoff;
-              ok = lx >= p.xoff && lx < p.TW + p.xoff && ty < p.TH && gy < p.H && gx < p.W;
-              pix = (long long)gy * p.W + gx;
-            } else {
-              pix = P.pix0 + j;
-              ok = pix < HW;
-            }
-            if (!ok || co >= p.Cout) continue;
-            float val = 0.f;
-            for (int k = 0; k < P.nslots; ++k) val += __ldcg(wst + ((long long)k * p.N + j) * CV_M + tid);
-            val += b;
-            if (zb) val += __ldg(zb + pix * p.zs_p);
-            if (p.relu_out) val = fmaxf(val, 0.f);
-            yb[pix * p.ys_p] = val;
+  // ================================== finish: all twelve warps ==================================
+  for (int pi = 0; pi < nparts; ++pi) {
+    const ConvPart& P = pi ? part1 : part0;
+    asm volatile("bar.sync 2, 384;" ::: "memory");          // direct: the tile is staged; shares: who stores it is known
+    const bool fin = T.last[pi] != 0;
+    if (!direct && fin) {
+      __threadfence();
+      if (staged_nchw) {
+        reduce_shares(P, warp, true);
+      } else if (p.cl_vec) {
+        reduce_shares(P, warp, false);
+      } else if (warp < 4) {                               // odd layouts: thread == channel, element-wise
+        const float* wst = p.ws + (P.tile_lin * p.maxslots) * (long long)(p.N * CV_M);
+        const int co = P.cot * CV_M + tid;
+        const float b = (p.bias && co < p.Cout) ? __ldg(p.bias + co) : 0.f;
+        float* yb = p.y + (long long)P.nb * p.ys_n + (long long)co * p.ys_c;
+        const float* zb = p.z ? p.z + (long long)P.nb * p.zs_n + (long long)co * p.zs_c : nullptr;
+        for (int j = 0; j < p.N; ++j) {
+          bool ok;
+          long long pix;
+          if (KS == 3) {
+            const int ty = j / TWp, lx = j - ty * TWp;
+            const int gy = P.ty0 + ty, gx = P.tx0 + lx - p.xoff;
+            ok = lx >= p.xoff && lx < p.TW + p.xoff && ty < p.TH && gy < p.H && gx < p.W;
+            pix = (long long)gy * p.W + gx;
+          } else {
+            pix = P.pix0 + j;
+            ok = pix < HW;
           }
+          if (!ok || co >= p.Cout) continue;
+          float val = 0.f;
+          for (int k = 0; k < P.nslots; ++k) val += __ldcg(wst + ((long long)k * p.N + j) * CV_M + tid);
+          val += b;
+          if (zb) val += __ldg(zb + pix * p.zs_p);
+          if (p.relu_out) val = fmaxf(val, 0.f);
+          yb[pix * p.ys_p] = val;
         }
       }
-      if (staged_nchw) {
-        if (!direct) asm volatile("bar.sync 2, 512;" ::: "memory");   // shares added up in the staging buffer
-        if (fin) store_staged_rows(P, warp);
-      } else if (direct && p.cl_vec) {
-        store_staged_rows(P, warp);
-      }
-      if (pi + 1 < nparts) asm volatile("bar.sync 2, 512;" ::: "memory");   // staging buffer free again
-      if (!direct && fin && tid == 0) p.counters[P.tile_lin] = 0;           // ready for the next launch
     }
+    if (staged_nchw) {
+      if (!direct) asm volatile("bar.sync 2, 384;" ::: "memory");   // shares added up in the staging buffer
+      if (fin) store_staged_rows(P, warp);
+    } else if (direct && p.cl_vec) {
+      store_staged_rows(P, warp);
+    }
+    if (pi + 1 < nparts) asm volatile("bar.sync 2, 384;" ::: "memory");   // staging buffer free again
+    if (!direct && fin && tid == 0) p.counters[P.tile_lin] = 0;           // ready for the next launch
   }
 }
 
