@@ -915,33 +915,39 @@ extern "C" int cutie_readout_gather(const int32_t* idx, const float* w, int64_t 
                                     const int64_t* seg_val_bstride, int64_t K, int64_t CV, float* out, void* stream) {
   CUTIE_REQUIRE(num_segments >= 1 && num_segments <= kMaxSeg, "1..4 segments");
   CUTIE_REQUIRE(CV == 256, "CV must be 256");
-  CUTIE_REQUIRE(K >= 1 && K <= 16, "1..16 objects per call");
+  CUTIE_REQUIRE(K >= 1, "at least one object");
   CUTIE_REQUIRE(kpad == 32 || kpad == 64, "kpad must be 32 or 64");
   CUTIE_REQUIRE(idx && w && out, "null argument");
-  GatherParams gp;
-  memset(&gp, 0, sizeof(gp));
-  long long tot = 0;
-  for (int s = 0; s < num_segments; ++s) {
-    gp.segs.begin[s] = tot;
-    tot += seg_len[s];
-    for (int k = 0; k < K; ++k) {
-      gp.segs.rows[s * K + k] = (const float*)seg_val[s * K + k];
-      gp.segs.bs[s * K + k] = seg_val_bstride[s * K + k];
+  // The kernel's parameter block holds the row pointers of at most kMaxObj objects.  Each output plane out[b, k]
+  // depends on object k alone, so larger calls launch once per group of kMaxObj objects with `out` offset by the
+  // group; `K` stays the full count, the batch stride of `out`.
+  for (long long k0 = 0; k0 < K; k0 += kMaxObj) {
+    const int nk = (int)(K - k0 < kMaxObj ? K - k0 : kMaxObj);
+    GatherParams gp;
+    memset(&gp, 0, sizeof(gp));
+    long long tot = 0;
+    for (int s = 0; s < num_segments; ++s) {
+      gp.segs.begin[s] = tot;
+      tot += seg_len[s];
+      for (int k = 0; k < nk; ++k) {
+        gp.segs.rows[s * nk + k] = (const float*)seg_val[s * K + k0 + k];
+        gp.segs.bs[s * nk + k] = seg_val_bstride[s * K + k0 + k];
+      }
     }
+    for (int s = num_segments; s <= kMaxSeg; ++s) gp.segs.begin[s] = tot;
+    gp.segs.nseg = num_segments;
+    gp.segs.nobj = nk;
+    gp.idx = idx;
+    gp.w = w;
+    gp.Q = Q;
+    gp.kpad = kpad;
+    gp.K = K;
+    gp.CV = CV;
+    gp.out = out + k0 * CV * Q;
+    dim3 grid((unsigned)((Q + GQ - 1) / GQ), (unsigned)nk, (unsigned)B);
+    readout_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(gp);
+    CUTIE_CHECK_LAUNCH();
   }
-  for (int s = num_segments; s <= kMaxSeg; ++s) gp.segs.begin[s] = tot;
-  gp.segs.nseg = num_segments;
-  gp.segs.nobj = (int)K;
-  gp.idx = idx;
-  gp.w = w;
-  gp.Q = Q;
-  gp.kpad = kpad;
-  gp.K = K;
-  gp.CV = CV;
-  gp.out = out;
-  dim3 grid((unsigned)((Q + GQ - 1) / GQ), (unsigned)K, (unsigned)B);
-  readout_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(gp);
-  CUTIE_CHECK_LAUNCH();
   return 0;
 }
 

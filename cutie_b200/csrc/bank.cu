@@ -88,14 +88,15 @@ struct ConsParams {
   long long pk_bs;
   const float* pe;
   long long pe_bs;
-  long long P, n_total, K;
-  float* out_val[16];
-  long long out_val_bs[16];
+  long long P, n_total, K;  // K: objects of THIS launch (at most kMaxObj)
+  float* out_val[kMaxObj];
+  long long out_val_bs[kMaxObj];
   float* out_shr;
   long long out_shr_bs;
   float* ws;  // [B][P][n_total]
   float* out_max;   // optional [B][P]: the softmax's max over the candidates (the per-shard affinity maximum of the sharded path)
   float* out_sum;   // optional [B][P]: sum_n exp(S[n,p] - max)
+  int readout_only; // phases 1-2 ran in an earlier launch of this call: ws holds exp(S - max); only the values are read out
 };
 
 __device__ __forceinline__ float block_reduce(float v, float* red, bool is_max) {
@@ -116,70 +117,82 @@ __global__ void __launch_bounds__(256) consolidate_kernel(const ConsParams p) {
   const int tid = threadIdx.x;
   const int b = blockIdx.y;
   const long long p0 = (long long)blockIdx.x * PT;
-  for (int i = tid; i < PT * 64; i += 256) {
-    int pp = i / 64, c = i % 64;
-    float e = 0.f, k = 0.f;
-    if (p0 + pp < p.P) {
-      e = p.pe[(long long)b * p.pe_bs + (p0 + pp) * 64 + c];
-      k = p.pk[(long long)b * p.pk_bs + (p0 + pp) * 64 + c];
-    }
-    float a = sqrtf(e);
-    a_s[pp][c] = a;
-    b_s[pp][c] = a * k;
-  }
-  __syncthreads();
   float* ws = p.ws + ((long long)b * p.P + p0) * p.n_total;
-  // phase 1: similarities of every candidate token against this CTA's prototypes
-  float lmax[PT];
+  if (p.readout_only) {
+    // A later object group: the first launch left exp(S - max) in ws.  The normaliser is summed again in the order and
+    // with the reduction of phase 2, so 1/se -- and every object's value rows -- are bit-identical to that launch's.
+    for (int pp = 0; pp < PT; ++pp) {
+      if (p0 + pp >= p.P) break;
+      float se = 0.f;
+      for (long long n = tid; n < p.n_total; n += 256) se += ws[(long long)pp * p.n_total + n];
+      se = block_reduce(se, red, false);
+      if (tid == 0) inv_sum[pp] = 1.f / se;
+    }
+  } else {
+    for (int i = tid; i < PT * 64; i += 256) {
+      int pp = i / 64, c = i % 64;
+      float e = 0.f, k = 0.f;
+      if (p0 + pp < p.P) {
+        e = p.pe[(long long)b * p.pe_bs + (p0 + pp) * 64 + c];
+        k = p.pk[(long long)b * p.pk_bs + (p0 + pp) * 64 + c];
+      }
+      float a = sqrtf(e);
+      a_s[pp][c] = a;
+      b_s[pp][c] = a * k;
+    }
+    __syncthreads();
+    // phase 1: similarities of every candidate token against this CTA's prototypes
+    float lmax[PT];
 #pragma unroll
-  for (int pp = 0; pp < PT; ++pp) lmax[pp] = -CUDART_INF_F;
-  for (long long n = tid; n < p.n_total; n += 256) {
-    const int s = seg_of(p.segs.begin, p.segs.nseg, n);
-    const float4* row = reinterpret_cast<const float4*>(p.segs.key[s] + (long long)b * p.segs.key_bs[s] +
-                                                        (n - p.segs.begin[s]) * 64);
-    const float shr = p.segs.shr[s][(long long)b * p.segs.shr_bs[s] + (n - p.segs.begin[s])];
-    float acc[PT];
+    for (int pp = 0; pp < PT; ++pp) lmax[pp] = -CUDART_INF_F;
+    for (long long n = tid; n < p.n_total; n += 256) {
+      const int s = seg_of(p.segs.begin, p.segs.nseg, n);
+      const float4* row = reinterpret_cast<const float4*>(p.segs.key[s] + (long long)b * p.segs.key_bs[s] +
+                                                          (n - p.segs.begin[s]) * 64);
+      const float shr = p.segs.shr[s][(long long)b * p.segs.shr_bs[s] + (n - p.segs.begin[s])];
+      float acc[PT];
 #pragma unroll
-    for (int pp = 0; pp < PT; ++pp) acc[pp] = 0.f;
+      for (int pp = 0; pp < PT; ++pp) acc[pp] = 0.f;
 #pragma unroll 4
-    for (int c4 = 0; c4 < 16; ++c4) {
-      const float4 kf = __ldg(row + c4);
+      for (int c4 = 0; c4 < 16; ++c4) {
+        const float4 kf = __ldg(row + c4);
+#pragma unroll
+        for (int pp = 0; pp < PT; ++pp) {
+          float d;
+          d = fmaf(a_s[pp][4 * c4 + 0], kf.x, -b_s[pp][4 * c4 + 0]); acc[pp] = fmaf(d, d, acc[pp]);
+          d = fmaf(a_s[pp][4 * c4 + 1], kf.y, -b_s[pp][4 * c4 + 1]); acc[pp] = fmaf(d, d, acc[pp]);
+          d = fmaf(a_s[pp][4 * c4 + 2], kf.z, -b_s[pp][4 * c4 + 2]); acc[pp] = fmaf(d, d, acc[pp]);
+          d = fmaf(a_s[pp][4 * c4 + 3], kf.w, -b_s[pp][4 * c4 + 3]); acc[pp] = fmaf(d, d, acc[pp]);
+        }
+      }
 #pragma unroll
       for (int pp = 0; pp < PT; ++pp) {
-        float d;
-        d = fmaf(a_s[pp][4 * c4 + 0], kf.x, -b_s[pp][4 * c4 + 0]); acc[pp] = fmaf(d, d, acc[pp]);
-        d = fmaf(a_s[pp][4 * c4 + 1], kf.y, -b_s[pp][4 * c4 + 1]); acc[pp] = fmaf(d, d, acc[pp]);
-        d = fmaf(a_s[pp][4 * c4 + 2], kf.z, -b_s[pp][4 * c4 + 2]); acc[pp] = fmaf(d, d, acc[pp]);
-        d = fmaf(a_s[pp][4 * c4 + 3], kf.w, -b_s[pp][4 * c4 + 3]); acc[pp] = fmaf(d, d, acc[pp]);
+        const float sv = -acc[pp] * shr * 0.125f;
+        if (p0 + pp < p.P) ws[(long long)pp * p.n_total + n] = sv;
+        lmax[pp] = fmaxf(lmax[pp], sv);
       }
     }
-#pragma unroll
+    // phase 2: softmax statistics + shrinkage readout
     for (int pp = 0; pp < PT; ++pp) {
-      const float sv = -acc[pp] * shr * 0.125f;
-      if (p0 + pp < p.P) ws[(long long)pp * p.n_total + n] = sv;
-      lmax[pp] = fmaxf(lmax[pp], sv);
-    }
-  }
-  // phase 2: softmax statistics + shrinkage readout
-  for (int pp = 0; pp < PT; ++pp) {
-    if (p0 + pp >= p.P) break;
-    const float mx = block_reduce(lmax[pp], red, true);
-    float se = 0.f, ss = 0.f;
-    for (long long n = tid; n < p.n_total; n += 256) {
-      const float e = expf(ws[(long long)pp * p.n_total + n] - mx);
-      ws[(long long)pp * p.n_total + n] = e;
-      const int s = seg_of(p.segs.begin, p.segs.nseg, n);
-      se += e;
-      ss += e * p.segs.shr[s][(long long)b * p.segs.shr_bs[s] + (n - p.segs.begin[s])];
-    }
-    se = block_reduce(se, red, false);
-    ss = block_reduce(ss, red, false);
-    if (tid == 0) {
-      inv_sum[pp] = 1.f / se;
-      p.out_shr[(long long)b * p.out_shr_bs + p0 + pp] = ss / se;
-      if (p.out_max) {
-        p.out_max[(long long)b * p.P + p0 + pp] = mx;
-        p.out_sum[(long long)b * p.P + p0 + pp] = se;
+      if (p0 + pp >= p.P) break;
+      const float mx = block_reduce(lmax[pp], red, true);
+      float se = 0.f, ss = 0.f;
+      for (long long n = tid; n < p.n_total; n += 256) {
+        const float e = expf(ws[(long long)pp * p.n_total + n] - mx);
+        ws[(long long)pp * p.n_total + n] = e;
+        const int s = seg_of(p.segs.begin, p.segs.nseg, n);
+        se += e;
+        ss += e * p.segs.shr[s][(long long)b * p.segs.shr_bs[s] + (n - p.segs.begin[s])];
+      }
+      se = block_reduce(se, red, false);
+      ss = block_reduce(ss, red, false);
+      if (tid == 0) {
+        inv_sum[pp] = 1.f / se;
+        p.out_shr[(long long)b * p.out_shr_bs + p0 + pp] = ss / se;
+        if (p.out_max) {
+          p.out_max[(long long)b * p.P + p0 + pp] = mx;
+          p.out_sum[(long long)b * p.P + p0 + pp] = se;
+        }
       }
     }
   }
@@ -284,7 +297,7 @@ extern "C" int cutie_consolidate_partial(int num_segments, const void* const* se
   CUTIE_REQUIRE((out_max == nullptr) == (out_sumexp == nullptr), "out_max and out_sumexp come together");
   CUTIE_REQUIRE(num_segments >= 1 && num_segments <= kMaxSeg, "1..4 segments");
   CUTIE_REQUIRE(CK == 64, "CK must be 64");
-  CUTIE_REQUIRE(K >= 0 && K <= 16, "0..16 objects");
+  CUTIE_REQUIRE(K >= 0, "negative object count");
   CUTIE_REQUIRE(K == 0 || CV == 256, "CV must be 256");
   CUTIE_REQUIRE(proto_key && proto_sel && out_shr && workspace && P >= 1 && B >= 1, "null/empty argument");
   ConsParams cp;
@@ -298,34 +311,42 @@ extern "C" int cutie_consolidate_partial(int num_segments, const void* const* se
     cp.segs.begin[s] = tot;
     cp.vals.begin[s] = tot;
     tot += seg_len[s];
-    for (int k = 0; k < K; ++k) {
-      cp.vals.rows[s * K + k] = (const float*)seg_val[s * K + k];
-      cp.vals.bs[s * K + k] = seg_val_bstride[s * K + k];
-    }
   }
   for (int s = num_segments; s <= kMaxSeg; ++s) cp.segs.begin[s] = cp.vals.begin[s] = tot;
   CUTIE_REQUIRE(tot == n_total && n_total >= 1, "n_total != sum of segment lengths");
   cp.segs.nseg = cp.vals.nseg = num_segments;
-  cp.vals.nobj = (int)K;
   cp.pk = proto_key;
   cp.pk_bs = pk_bstride;
   cp.pe = proto_sel;
   cp.pe_bs = ps_bstride;
   cp.P = P;
   cp.n_total = n_total;
-  cp.K = K;
-  for (int k = 0; k < K; ++k) {
-    cp.out_val[k] = (float*)out_val[k];
-    cp.out_val_bs[k] = out_val_bstride[k];
-  }
   cp.out_shr = out_shr;
   cp.out_shr_bs = out_shr_bstride;
   cp.ws = workspace;
   cp.out_max = out_max;
   cp.out_sum = out_sumexp;
   dim3 grid((unsigned)((P + PT - 1) / PT), (unsigned)B);
-  consolidate_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(cp);
-  CUTIE_CHECK_LAUNCH();
+  // One launch per group of at most kMaxObj objects.  The first computes the similarities and softmax statistics (the
+  // bulk of the work: P x n_total x 64 FMAs) and reads out its objects; later groups reuse the exp(S - max) it left in the
+  // workspace and only read out their values.
+  for (long long k0 = 0; k0 == 0 || k0 < K; k0 += kMaxObj) {
+    const int nk = (int)(K - k0 < kMaxObj ? K - k0 : kMaxObj);
+    for (int s = 0; s < num_segments; ++s)
+      for (int k = 0; k < nk; ++k) {
+        cp.vals.rows[s * nk + k] = (const float*)seg_val[s * K + k0 + k];
+        cp.vals.bs[s * nk + k] = seg_val_bstride[s * K + k0 + k];
+      }
+    cp.vals.nobj = nk;
+    cp.K = nk;
+    for (int k = 0; k < nk; ++k) {
+      cp.out_val[k] = (float*)out_val[k0 + k];
+      cp.out_val_bs[k] = out_val_bstride[k0 + k];
+    }
+    cp.readout_only = k0 > 0;
+    consolidate_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(cp);
+    CUTIE_CHECK_LAUNCH();
+  }
   return 0;
 }
 

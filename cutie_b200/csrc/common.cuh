@@ -44,9 +44,13 @@ struct KeySegments {
   int nseg;
 };
 
+// Objects per launch of the kernels that take per-object row pointers by value (readout gather, consolidation).
+// Their C entry points accept any number of objects and launch once per group of at most kMaxObj.
+constexpr int kMaxObj = 16;
+
 struct RowSegments {
-  const float* rows[kMaxSeg * 16];  // [segment][object]
-  long long bs[kMaxSeg * 16];
+  const float* rows[kMaxSeg * kMaxObj];  // [segment][object]
+  long long bs[kMaxSeg * kMaxObj];
   long long begin[kMaxSeg + 1];
   int nseg;
   int nobj;

@@ -298,6 +298,66 @@ __global__ void __launch_bounds__(256) qt_aux_mask_kernel(const float* __restric
   }
 }
 
+// The same computation for K > AUX_MAX_K, where a pixel's K logits no longer fit in registers.  The objects go through
+// the 8 warps in groups of AUX_MAX_K; warp 0 writes each group's logits to `logits` and folds them into prod(1 - p).
+// Two more passes over k re-read the pixel's own logits: the log-odds maximum, then the foreground test.  Every value
+// is formed by the same operations in the same order as in qt_aux_mask_kernel, so a pixel's decision does not depend
+// on which of the two kernels ran.
+__device__ __forceinline__ float aux_log_odds(float v) {
+  const float pr = fminf(fmaxf(1.f / (1.f + expf(-v)), 1e-7f), 1.f - 1e-7f);
+  return logf(pr / (1.f - pr));
+}
+
+__global__ void __launch_bounds__(256) qt_aux_mask_stream_kernel(const float* __restrict__ pixel,
+                                                                 const float* __restrict__ w,
+                                                                 const float* __restrict__ bias, long long K,
+                                                                 long long HW, float* __restrict__ logits,
+                                                                 uint8_t* __restrict__ fg, int* __restrict__ fg_count) {
+  __shared__ float part[AUX_MAX_K][8][33];
+  __shared__ float wsm[E_];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long b = blockIdx.y, px = (long long)blockIdx.x * 32 + lane;
+  const bool live = px < HW;
+  wsm[tid] = w[tid];
+  __syncthreads();
+  float bgp = 1.f;
+  for (long long k0 = 0; k0 < K; k0 += AUX_MAX_K) {
+    const int nk = (int)(K - k0 < AUX_MAX_K ? K - k0 : AUX_MAX_K);
+    for (int k = 0; k < nk; ++k) {
+      const float* base = pixel + ((b * K + k0 + k) * E_ + warp * 32) * HW;
+      float acc = 0.f;
+      if (live) {
+#pragma unroll 8
+        for (int c = 0; c < 32; ++c) acc = fmaf(wsm[warp * 32 + c], fmaxf(base[(long long)c * HW + px], 0.f), acc);
+      }
+      part[k][warp][lane] = acc;
+    }
+    __syncthreads();
+    if (warp == 0) {
+      for (int k = 0; k < nk; ++k) {
+        float v = bias[0];
+#pragma unroll
+        for (int g = 0; g < 8; ++g) v += part[k][g][lane];
+        if (live) logits[(b * K + k0 + k) * HW + px] = v;
+        const float pr = 1.f / (1.f + expf(-v));
+        bgp *= (1.f - pr);
+      }
+    }
+    __syncthreads();   // part is refilled by the next group
+  }
+  if (warp != 0) return;
+  const float bc = fminf(fmaxf(bgp, 1e-7f), 1.f - 1e-7f);
+  float mx = logf(bc / (1.f - bc));
+  for (long long k = 0; k < K; ++k)
+    if (live) mx = fmaxf(mx, aux_log_odds(logits[(b * K + k) * HW + px]));
+  for (long long k = 0; k < K; ++k) {
+    const bool f = live && aux_log_odds(logits[(b * K + k) * HW + px]) >= mx;
+    if (live) fg[(b * K + k) * HW + px] = f ? 1 : 0;
+    const unsigned m = __ballot_sync(0xffffffffu, f);
+    if (lane == 0 && m) atomicAdd(&fg_count[b * K + k], __popc(m));
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // The query-side chain of a transformer block as ONE launch.  Between the two tensor-core cross attentions a block runs
 // ~12 skinny ops on the [objects x 16, 256] query tile (combine, out-proj, LayerNorm + q/k/v projections, 16 x 16 self
@@ -454,9 +514,12 @@ extern "C" int cutie_qt_aux_mask(const float* pixel, const float* w, const float
                                  int64_t HW, float* logits, uint8_t* fg, int32_t* fg_count, void* stream) {
   CUTIE_REQUIRE(pixel && w && b && logits && fg && fg_count, "null argument");
   CUTIE_REQUIRE(E == E_, "embed_dim must be 256");
-  CUTIE_REQUIRE(K >= 1 && K <= AUX_MAX_K && B >= 1 && HW >= 1, "1..32 objects");
+  CUTIE_REQUIRE(K >= 1 && B >= 1 && HW >= 1, "empty argument");
   dim3 grid((unsigned)((HW + 31) / 32), (unsigned)B);
-  qt_aux_mask_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(pixel, w, b, K, HW, logits, fg, fg_count);
+  if (K <= AUX_MAX_K)
+    qt_aux_mask_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(pixel, w, b, K, HW, logits, fg, fg_count);
+  else
+    qt_aux_mask_stream_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(pixel, w, b, K, HW, logits, fg, fg_count);
   CUTIE_CHECK_LAUNCH();
   return 0;
 }

@@ -291,7 +291,9 @@ def topk_merge(part_val: torch.Tensor, part_idx: torch.Tensor, top_k: int, n_tot
 
 def readout_gather(idx: torch.Tensor, w: torch.Tensor, segments: Sequence[BankSegment],
                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[b,k,c,q] = sum_j w[b,q,j] * V_k[idx[b,q,j], c]  ->  [B, K, CV, Q] (a6, evaluated sparsely)."""
+    """out[b,k,c,q] = sum_j w[b,q,j] * V_k[idx[b,q,j], c]  ->  [B, K, CV, Q] (a6, evaluated sparsely).
+    Any number of objects K >= 1: one kernel launch per group of 16, and object k's plane is the same bits as in a
+    call with object k alone."""
     B, Q, kpad = idx.shape
     K = len(segments[0].values)
     CV = segments[0].values[0].shape[2]
@@ -307,7 +309,7 @@ def readout_gather(idx: torch.Tensor, w: torch.Tensor, segments: Sequence[BankSe
             strides.append(v.stride(0))
     PA, IA, IS = ctypes.c_void_p * (ns * K), ctypes.c_int64 * (ns * K), ctypes.c_int64 * ns
     _L = lib()
-    with _call('readout_gather', 1):
+    with _call('readout_gather', -(-K // 16)):
         st = _L.cutie_readout_gather(_ptr(idx, torch.int32), _ptr(w), _i64(B), _i64(Q), ctypes.c_int(kpad),
                                         ctypes.c_int(ns), IS(*[s.n for s in segments]), PA(*ptrs), IA(*strides),
                                         _i64(K), _i64(CV), _ptr(out), _stream())
@@ -674,6 +676,8 @@ def consolidate(segments: Sequence[BankSegment], proto_key: torch.Tensor, proto_
     proto_key, proto_sel: [B, P, CK] token-major.  out_values[k]: [B, P, CV] rows; out_shrinkage [B, P].
     stats = (out_max, out_sumexp), both [B, P] dense (key-sharded memory): the softmax statistics of THIS shard of the
     candidates, by which its results are normalised -- what the shards exchange to combine them (inference/sharded.py).
+    Any number of objects K >= 0: the similarities and softmax statistics are computed once, the value readout runs
+    once per group of 16 objects, and object k's rows are the same bits as in a call with object k alone.
     """
     B, P, CK = proto_key.shape
     ns = len(segments)
@@ -692,7 +696,7 @@ def consolidate(segments: Sequence[BankSegment], proto_key: torch.Tensor, proto_
     if stats is not None:
         for t in stats:
             assert t.shape == (B, P) and t.is_contiguous() and t.dtype == torch.float32
-    with _call('consolidate', 1):
+    with _call('consolidate', max(1, -(-K // 16))):
         st = lib().cutie_consolidate_partial(
             ctypes.c_int(ns), PA(*[s.key.data_ptr() for s in segments]), PA(*[s.shrinkage.data_ptr() for s in segments]),
             IA(*[s.n for s in segments]), IA(*[s.key.stride(0) for s in segments]),
@@ -778,7 +782,9 @@ def qt_self_attention(qk: torch.Tensor, v: torch.Tensor, num_queries: int, num_h
 
 def qt_aux_mask(pixel: torch.Tensor, w: torch.Tensor, b: torch.Tensor, B: int, K: int):
     """mask_pred + sigmoid + aggregate + foreground test (a15) in one pass over pixel [B*K, E, HW].
-    Returns (aux_logits f32 [B,K,HW], fg uint8 [B,K,HW], fg_count int32 [B*K])."""
+    Returns (aux_logits f32 [B,K,HW], fg uint8 [B,K,HW], fg_count int32 [B*K]).
+    Any number of objects K >= 1.  Above 32 a second kernel form streams over the objects instead of holding a pixel's
+    K logits in registers; it forms every value in the same order, so a pixel's foreground decision is the same."""
     BK, E, HW = pixel.shape
     assert pixel.is_contiguous(), 'pixel must be channel-major contiguous [B*K, E, HW]'
     dev = pixel.device

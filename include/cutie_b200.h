@@ -108,7 +108,8 @@ int cutie_topk_merge(const float* part_val, const int32_t* part_idx, int64_t B, 
 /* Sparse value readout out[b,k,c,q] = sum_j w[b,q,j] * V_k[idx[b,q,j], c].
  * Replaces MemoryManager._readout (memory_manager.py:77-88; dense [K*CV,N]x[N,Q] GEMM against a matrix
  * with top_k non-zeros per column) and _get_visual_values_by_ids (:101-110; torch.stack/cat of the whole
- * value bank every frame).  seg_val[s*K + k] -> token-major values of object k in segment s. */
+ * value bank every frame).  seg_val[s*K + k] -> token-major values of object k in segment s.  Any K >= 1: the call
+ * launches once per group of at most 16 objects, and out[b,k] is bit-identical to a call with object k alone. */
 int cutie_readout_gather(const int32_t* idx, const float* w, int64_t B, int64_t Q, int kpad, int num_segments,
                          const int64_t* seg_len, const void* const* seg_val, const int64_t* seg_val_bstride,
                          int64_t K, int64_t CV, float* out, void* stream);
@@ -250,7 +251,9 @@ int cutie_bank_gather(int num_segments, const void* const* seg_rows, const int64
                       int64_t B, int64_t m, int64_t C, void* stream);
 /* Long-term potentiation: for every prototype p, A[:,p] = softmax_n(S[n,p]) over ALL candidate tokens
  * (max-subtracted, memory_utils.py:68-71), out_val_k[b,p,:] = sum_n A[n,p] V_k[n,:], out_shr[b,p] = sum_n A[n,p] shr[n].
- * Replaces MemoryManager.consolidation (memory_manager.py:345-356).  workspace: B*P*n_total floats. */
+ * Replaces MemoryManager.consolidation (memory_manager.py:345-356).  workspace: B*P*n_total floats.  Any K >= 0: the
+ * similarities and softmax statistics are computed once per call; the value readout runs once per group of at most 16
+ * objects, and out_val[k] is bit-identical to a call with object k alone. */
 int cutie_consolidate(int num_segments, const void* const* seg_key, const void* const* seg_shrinkage,
                       const int64_t* seg_len, const int64_t* seg_key_bstride, const int64_t* seg_shr_bstride,
                       const void* const* seg_val, const int64_t* seg_val_bstride, int64_t K,
@@ -321,7 +324,8 @@ int cutie_qt_chain(const cutie_qt_op* ops, int nops, const void* const* prefetch
                    int nprefetch, uint32_t* sync_ws, void* stream);
 /* mask_pred 1x1 conv on relu(pixel) + sigmoid + aggregate + foreground test + per-object foreground count.
  * Replaces mask_pred[i] and QueryTransformer._get_aux_mask (object_transformer.py:153-155,165-167,179-205;
- * cutie/utils/tensor_utils.py:47-54).  The [(B*K*heads),Q,HW] bool mask is represented by fg + fg_count. */
+ * cutie/utils/tensor_utils.py:47-54).  The [(B*K*heads),Q,HW] bool mask is represented by fg + fg_count.  Any K >= 1;
+ * above 32 objects a streaming form runs the same floating-point operations in the same order. */
 int cutie_qt_aux_mask(const float* pixel, const float* w, const float* b, int64_t B, int64_t K, int64_t E,
                       int64_t HW, float* logits, uint8_t* fg, int32_t* fg_count, void* stream);
 /* read_from_pixel attention core (masked, queries <- pixels) on the tensor cores (wgmma) (3xTF32, fp32-class accuracy):
