@@ -510,6 +510,11 @@ def conv_tc(x: torch.Tensor, weight_image: torch.Tensor, bias: Optional[torch.Te
     if weight_image.numel() * weight_image.element_size() != conv_weight_image_bytes(cout, Cin, ksize, f16):
         raise KernelError(f'conv_tc: the weight image does not fit a {ksize}x{ksize} {Cin}->{cout} layer in '
                           f'{"fp16" if f16 else "3xTF32"} form (build it with conv_weight_image{"_f16" if f16 else ""})')
+    if bias is not None:
+        # the kernel reads bias[0 .. cout) as dense floats: a view with a stride would be read as if it had none
+        if tuple(bias.shape) != (cout,) or bias.dtype != torch.float32:
+            raise KernelError(f'conv_tc: bias must be float32 of shape ({cout},), got {bias.dtype} {tuple(bias.shape)}')
+        bias = bias.detach().contiguous()
     cl = x.is_contiguous(memory_format=torch.channels_last) and not x.is_contiguous()
     if not cl:
         x = x.contiguous()
@@ -536,7 +541,7 @@ def conv_tc(x: torch.Tensor, weight_image: torch.Tensor, bias: Optional[torch.Te
     name = 'conv_tc_f16' if f16 else 'conv_tc'
     with _call(name, 1):
         st = getattr(lib(), 'cutie_' + name)(
-            _ptr(x), arr(_ncp_strides(x)), _ptr(weight_image), _ptr(bias.detach() if bias is not None else None),
+            _ptr(x), arr(_ncp_strides(x)), _ptr(weight_image), _ptr(bias),
             _ptr(residual), arr(zs) if zs is not None else None, _i64(N), _i64(Cin), _i64(cout), _i64(H), _i64(W),
             int(ksize), int(stride), int(bool(relu_in)), int(bool(relu_out)), _ptr(out), arr(_ncp_strides(out)), q,
             _ptr(ws), _ptr(cnt, torch.int32), _stream())

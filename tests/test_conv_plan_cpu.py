@@ -72,3 +72,15 @@ def test_3x3_tile_shape_fits_the_activation_stage(H, W):
     th, tw, n = tuple(out)
     assert th >= 1 and tw >= 1 and n % 16 == 0 and th * (tw + 2) <= n <= 128
     assert n + 2 * (tw + 2) + 2 <= 248                       # rows of the local padded grid + slack (CV3_ROWS)
+
+
+def test_3x3_boundary_widths_of_the_gpu_tests_straddle_a_tile_shape_change():
+    """tests/test_gpu_conv_tc.py runs 30 x 57 and 30 x 58 to cover both sides of a change of tile shape: one whole-row
+    column tile per row, then two column tiles."""
+    import cutie_b200.kernels as K_
+    out = (ctypes.c_int * 3)()
+    shapes = []
+    for W in (57, 58):
+        assert K_.lib().cutie_debug_conv_tile_shape(ctypes.c_int64(30), ctypes.c_int64(W), out) == 0
+        shapes.append(tuple(out))
+    assert shapes[0][1] == 57 and shapes[1][1] < 58, shapes
