@@ -245,19 +245,20 @@ __global__ void __launch_bounds__(256) qt_self_attention_kernel(const float* __r
 // ------------------------------------------------------------------------------------------------
 // mask_pred + sigmoid + aggregate + foreground test.  grid (ceil(HW/32), B), block 256:
 // lane == pixel, warp == group of 32 channels.
+//
+// Every kernel of this family forms its values through the device functions below, in the same order, so the logits and
+// a pixel's foreground decision are the same bits whichever kernel ran: the fused forms (cutie_qt_aux_mask) or the split
+// pair (cutie_qt_mask_logits, then cutie_qt_aux_fg over all objects' logits -- object sharding, where each rank computes
+// the logits of its own objects and the foreground test needs everyone's).
 constexpr int AUX_MAX_K = 32;
-__global__ void __launch_bounds__(256) qt_aux_mask_kernel(const float* __restrict__ pixel, const float* __restrict__ w,
-                                                          const float* __restrict__ bias, long long K, long long HW,
-                                                          float* __restrict__ logits, uint8_t* __restrict__ fg,
-                                                          int* __restrict__ fg_count) {
-  __shared__ float part[AUX_MAX_K][8][33];
-  __shared__ float wsm[E_];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const long long b = blockIdx.y, px = (long long)blockIdx.x * 32 + lane;
-  wsm[tid] = w[tid];
-  __syncthreads();
-  for (int k = 0; k < K; ++k) {
-    const float* base = pixel + ((b * K + k) * E_ + warp * 32) * HW;
+typedef float AuxPart[8][33];
+
+// part[k][warp][lane] = the warp's 32-channel share of mask_pred's dot product for objects k0 .. k0 + nk - 1
+__device__ __forceinline__ void aux_partials(const float* __restrict__ pixel, const float* wsm, long long b, long long K,
+                                             long long k0, int nk, long long HW, long long px, int warp, int lane,
+                                             AuxPart* part) {
+  for (int k = 0; k < nk; ++k) {
+    const float* base = pixel + ((b * K + k0 + k) * E_ + warp * 32) * HW;
     float acc = 0.f;
     if (px < HW) {
 #pragma unroll 8
@@ -265,55 +266,80 @@ __global__ void __launch_bounds__(256) qt_aux_mask_kernel(const float* __restric
     }
     part[k][warp][lane] = acc;
   }
+}
+
+__device__ __forceinline__ float aux_logit(const AuxPart* part, int k, int lane, float bias) {
+  float v = bias;
+#pragma unroll
+  for (int g = 0; g < 8; ++g) v += part[k][g][lane];
+  return v;
+}
+
+// the background probability prod(1 - p) folds in one object's logit
+__device__ __forceinline__ float aux_fold_bg(float bgp, float v) {
+  const float pr = 1.f / (1.f + expf(-v));
+  return bgp * (1.f - pr);
+}
+
+// log-odds after clamping to [1e-7, 1-1e-7] (tensor_utils.py:50-52): of an object's logit, and of the background
+__device__ __forceinline__ float aux_log_odds(float v) {
+  const float pr = fminf(fmaxf(1.f / (1.f + expf(-v)), 1e-7f), 1.f - 1e-7f);
+  return logf(pr / (1.f - pr));
+}
+__device__ __forceinline__ float aux_bg_log_odds(float bgp) {
+  const float bc = fminf(fmaxf(bgp, 1e-7f), 1.f - 1e-7f);
+  return logf(bc / (1.f - bc));
+}
+
+// one object's foreground flag of this warp's 32 pixels, and its count
+__device__ __forceinline__ void aux_emit(bool live, bool f, uint8_t* fg, int* fg_count, int lane) {
+  if (live) *fg = f ? 1 : 0;
+  const unsigned m = __ballot_sync(0xffffffffu, f);
+  if (lane == 0 && m) atomicAdd(fg_count, __popc(m));
+}
+
+__global__ void __launch_bounds__(256) qt_aux_mask_kernel(const float* __restrict__ pixel, const float* __restrict__ w,
+                                                          const float* __restrict__ bias, long long K, long long HW,
+                                                          float* __restrict__ logits, uint8_t* __restrict__ fg,
+                                                          int* __restrict__ fg_count) {
+  __shared__ AuxPart part[AUX_MAX_K];
+  __shared__ float wsm[E_];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long b = blockIdx.y, px = (long long)blockIdx.x * 32 + lane;
+  const bool live = px < HW;
+  wsm[tid] = w[tid];
+  __syncthreads();
+  aux_partials(pixel, wsm, b, K, 0, (int)K, HW, px, warp, lane, part);
   __syncthreads();
   if (warp == 0) {
     float lg[AUX_MAX_K];
     float bgp = 1.f;
     for (int k = 0; k < K; ++k) {
-      float v = bias[0];
-#pragma unroll
-      for (int g = 0; g < 8; ++g) v += part[k][g][lane];
-      lg[k] = v;
-      const float pr = 1.f / (1.f + expf(-v));
-      bgp *= (1.f - pr);
+      lg[k] = aux_logit(part, k, lane, bias[0]);
+      bgp = aux_fold_bg(bgp, lg[k]);
     }
-    // log-odds after clamping to [1e-7, 1-1e-7] (tensor_utils.py:50-52)
-    const float bc = fminf(fmaxf(bgp, 1e-7f), 1.f - 1e-7f);
-    float mx = logf(bc / (1.f - bc));
+    float mx = aux_bg_log_odds(bgp);
     float lo[AUX_MAX_K];
     for (int k = 0; k < K; ++k) {
-      const float pr = fminf(fmaxf(1.f / (1.f + expf(-lg[k])), 1e-7f), 1.f - 1e-7f);
-      lo[k] = logf(pr / (1.f - pr));
+      lo[k] = aux_log_odds(lg[k]);
       mx = fmaxf(mx, lo[k]);
     }
     for (int k = 0; k < K; ++k) {
-      const bool f = (px < HW) && (lo[k] >= mx);
-      if (px < HW) {
-        logits[(b * K + k) * HW + px] = lg[k];
-        fg[(b * K + k) * HW + px] = f ? 1 : 0;
-      }
-      const unsigned m = __ballot_sync(0xffffffffu, f);
-      if (lane == 0 && m) atomicAdd(&fg_count[b * K + k], __popc(m));
+      if (live) logits[(b * K + k) * HW + px] = lg[k];
+      aux_emit(live, live && lo[k] >= mx, fg + (b * K + k) * HW + px, &fg_count[b * K + k], lane);
     }
   }
 }
 
 // The same computation for K > AUX_MAX_K, where a pixel's K logits no longer fit in registers.  The objects go through
 // the 8 warps in groups of AUX_MAX_K; warp 0 writes each group's logits to `logits` and folds them into prod(1 - p).
-// Two more passes over k re-read the pixel's own logits: the log-odds maximum, then the foreground test.  Every value
-// is formed by the same operations in the same order as in qt_aux_mask_kernel, so a pixel's decision does not depend
-// on which of the two kernels ran.
-__device__ __forceinline__ float aux_log_odds(float v) {
-  const float pr = fminf(fmaxf(1.f / (1.f + expf(-v)), 1e-7f), 1.f - 1e-7f);
-  return logf(pr / (1.f - pr));
-}
-
+// Two more passes over k re-read the pixel's own logits: the log-odds maximum, then the foreground test.
 __global__ void __launch_bounds__(256) qt_aux_mask_stream_kernel(const float* __restrict__ pixel,
                                                                  const float* __restrict__ w,
                                                                  const float* __restrict__ bias, long long K,
                                                                  long long HW, float* __restrict__ logits,
                                                                  uint8_t* __restrict__ fg, int* __restrict__ fg_count) {
-  __shared__ float part[AUX_MAX_K][8][33];
+  __shared__ AuxPart part[AUX_MAX_K];
   __shared__ float wsm[E_];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const long long b = blockIdx.y, px = (long long)blockIdx.x * 32 + lane;
@@ -323,38 +349,70 @@ __global__ void __launch_bounds__(256) qt_aux_mask_stream_kernel(const float* __
   float bgp = 1.f;
   for (long long k0 = 0; k0 < K; k0 += AUX_MAX_K) {
     const int nk = (int)(K - k0 < AUX_MAX_K ? K - k0 : AUX_MAX_K);
-    for (int k = 0; k < nk; ++k) {
-      const float* base = pixel + ((b * K + k0 + k) * E_ + warp * 32) * HW;
-      float acc = 0.f;
-      if (live) {
-#pragma unroll 8
-        for (int c = 0; c < 32; ++c) acc = fmaf(wsm[warp * 32 + c], fmaxf(base[(long long)c * HW + px], 0.f), acc);
-      }
-      part[k][warp][lane] = acc;
-    }
+    aux_partials(pixel, wsm, b, K, k0, nk, HW, px, warp, lane, part);
     __syncthreads();
     if (warp == 0) {
       for (int k = 0; k < nk; ++k) {
-        float v = bias[0];
-#pragma unroll
-        for (int g = 0; g < 8; ++g) v += part[k][g][lane];
+        const float v = aux_logit(part, k, lane, bias[0]);
         if (live) logits[(b * K + k0 + k) * HW + px] = v;
-        const float pr = 1.f / (1.f + expf(-v));
-        bgp *= (1.f - pr);
+        bgp = aux_fold_bg(bgp, v);
       }
     }
     __syncthreads();   // part is refilled by the next group
   }
   if (warp != 0) return;
-  const float bc = fminf(fmaxf(bgp, 1e-7f), 1.f - 1e-7f);
-  float mx = logf(bc / (1.f - bc));
+  float mx = aux_bg_log_odds(bgp);
   for (long long k = 0; k < K; ++k)
     if (live) mx = fmaxf(mx, aux_log_odds(logits[(b * K + k) * HW + px]));
+  for (long long k = 0; k < K; ++k)
+    aux_emit(live, live && aux_log_odds(logits[(b * K + k) * HW + px]) >= mx, fg + (b * K + k) * HW + px,
+             &fg_count[b * K + k], lane);
+}
+
+// First half of the split form: the logits alone, [B, K, HW] for the K objects of `pixel`.
+__global__ void __launch_bounds__(256) qt_mask_logits_kernel(const float* __restrict__ pixel, const float* __restrict__ w,
+                                                             const float* __restrict__ bias, long long K, long long HW,
+                                                             float* __restrict__ logits) {
+  __shared__ AuxPart part[AUX_MAX_K];
+  __shared__ float wsm[E_];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long b = blockIdx.y, px = (long long)blockIdx.x * 32 + lane;
+  wsm[tid] = w[tid];
+  __syncthreads();
+  for (long long k0 = 0; k0 < K; k0 += AUX_MAX_K) {
+    const int nk = (int)(K - k0 < AUX_MAX_K ? K - k0 : AUX_MAX_K);
+    aux_partials(pixel, wsm, b, K, k0, nk, HW, px, warp, lane, part);
+    __syncthreads();
+    if (warp == 0 && px < HW)
+      for (int k = 0; k < nk; ++k) logits[(b * K + k0 + k) * HW + px] = aux_logit(part, k, lane, bias[0]);
+    __syncthreads();
+  }
+}
+
+// Second half: the foreground test of the objects at positions pos[0 .. n) of all K objects' logits [B, K, HW].
+// grid (ceil(HW/256), B), block 256, thread == pixel.  Up to AUX_MAX_K objects a pixel's logits and log-odds stay in
+// registers (REG); above, the pixel's logits are re-read for each pass, as in qt_aux_mask_stream_kernel.
+template <bool REG>
+__global__ void __launch_bounds__(256) qt_aux_fg_kernel(const float* __restrict__ logits, const int* __restrict__ pos,
+                                                        long long K, long long n, long long HW, uint8_t* __restrict__ fg,
+                                                        int* __restrict__ fg_count) {
+  const int lane = threadIdx.x & 31;
+  const long long b = blockIdx.y, px = (long long)blockIdx.x * 256 + threadIdx.x;
+  const bool live = px < HW;
+  const float* lp = logits + b * K * HW + (live ? px : 0);
+  float lo[REG ? AUX_MAX_K : 1];
+  float bgp = 1.f;
+  for (long long k = 0; k < K; ++k) bgp = aux_fold_bg(bgp, lp[k * HW]);
+  float mx = aux_bg_log_odds(bgp);
   for (long long k = 0; k < K; ++k) {
-    const bool f = live && aux_log_odds(logits[(b * K + k) * HW + px]) >= mx;
-    if (live) fg[(b * K + k) * HW + px] = f ? 1 : 0;
-    const unsigned m = __ballot_sync(0xffffffffu, f);
-    if (lane == 0 && m) atomicAdd(&fg_count[b * K + k], __popc(m));
+    const float l = aux_log_odds(lp[k * HW]);
+    if (REG) lo[k] = l;
+    mx = fmaxf(mx, l);
+  }
+  for (long long j = 0; j < n; ++j) {
+    const int k = pos[j];
+    const float l = REG ? lo[k] : aux_log_odds(lp[(long long)k * HW]);
+    aux_emit(live, live && l >= mx, fg + (b * n + j) * HW + px, &fg_count[b * n + j], lane);
   }
 }
 
@@ -520,6 +578,31 @@ extern "C" int cutie_qt_aux_mask(const float* pixel, const float* w, const float
     qt_aux_mask_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(pixel, w, b, K, HW, logits, fg, fg_count);
   else
     qt_aux_mask_stream_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(pixel, w, b, K, HW, logits, fg, fg_count);
+  CUTIE_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int cutie_qt_mask_logits(const float* pixel, const float* w, const float* b, int64_t B, int64_t K, int64_t E,
+                                    int64_t HW, float* logits, void* stream) {
+  CUTIE_REQUIRE(pixel && w && b && logits, "null argument");
+  CUTIE_REQUIRE(E == E_, "embed_dim must be 256");
+  CUTIE_REQUIRE(K >= 1 && B >= 1 && HW >= 1, "empty argument");
+  qt_mask_logits_kernel<<<dim3((unsigned)((HW + 31) / 32), (unsigned)B), 256, 0, (cudaStream_t)stream>>>(pixel, w, b, K,
+                                                                                                        HW, logits);
+  CUTIE_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int cutie_qt_aux_fg(const float* logits, const int32_t* positions, int64_t B, int64_t K, int64_t n,
+                               int64_t HW, uint8_t* fg, int32_t* fg_count, void* stream) {
+  CUTIE_REQUIRE(logits && positions && fg && fg_count, "null argument");
+  CUTIE_REQUIRE(K >= 1 && B >= 1 && HW >= 1 && n >= 1, "empty argument");
+  CUTIE_REQUIRE(n <= K, "more positions than objects");
+  dim3 grid((unsigned)((HW + 255) / 256), (unsigned)B);
+  if (K <= AUX_MAX_K)
+    qt_aux_fg_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(logits, positions, K, n, HW, fg, fg_count);
+  else
+    qt_aux_fg_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(logits, positions, K, n, HW, fg, fg_count);
   CUTIE_CHECK_LAUNCH();
   return 0;
 }

@@ -123,7 +123,18 @@ class EncoderLookahead:
 
 class InferenceCore:
     def __init__(self, network, cfg, *, image_feature_store: ImageFeatureStore = None,
-                 use_cuda_graphs: bool = False, memory_shard_group=None):
+                 use_cuda_graphs: bool = False, memory_shard_group=None, object_shard_group=None):
+        """memory_shard_group: split the memory bank's tokens over the group's ranks (MemoryManager).
+        object_shard_group: split the video's objects over the group's ranks (object_shards.py): each object's readout,
+        fusion, object transformer, decoder and mask encoder run on the rank that owns it.  Every rank of either group
+        calls step() with the same arguments and gets the same full result."""
+        if object_shard_group is not None:
+            if memory_shard_group is not None:
+                raise ValueError('object sharding cannot be combined with memory (key) sharding')
+            if cfg.chunk_size >= 1:
+                raise NotImplementedError('object sharding needs chunk_size < 1: chunks would couple objects per chunk')
+            if cfg.save_aux:
+                raise NotImplementedError('object sharding does not export auxiliary outputs (save_aux)')
         self.network = network
         self.cfg = cfg
         self.mem_every = cfg.mem_every
@@ -142,7 +153,12 @@ class InferenceCore:
             self.stagger_ti = set(np.round(np.linspace(1, self.mem_every, stagger)).astype(int))
         self.object_manager = ObjectManager()
         self.memory_shard_group = memory_shard_group
-        self.memory = MemoryManager(cfg=cfg, object_manager=self.object_manager, shard_group=memory_shard_group)
+        self.object_shards = None
+        if object_shard_group is not None:
+            from cutie_b200.inference.object_shards import ObjectShards
+            self.object_shards = ObjectShards(object_shard_group)
+        self.memory = MemoryManager(cfg=cfg, object_manager=self.object_manager, shard_group=memory_shard_group,
+                                    object_shards=self.object_shards)
         self.image_feature_store = image_feature_store or ImageFeatureStore(self.network)
         self.last_mask = None
         self.last_logits = None      # network.segment(...)[1] of the latest segmented frame (parity hook)
@@ -161,7 +177,7 @@ class InferenceCore:
     def clear_memory(self):
         self._reset_clock()
         self.memory = MemoryManager(cfg=self.cfg, object_manager=self.object_manager,
-                                    shard_group=self.memory_shard_group)
+                                    shard_group=self.memory_shard_group, object_shards=self.object_shards)
 
     def clear_non_permanent_memory(self):
         self._reset_clock()
@@ -183,6 +199,9 @@ class InferenceCore:
             log.warning('Trying to add an empty object mask to memory!')
             return
         ids = self.object_manager.all_obj_ids
+        if self.object_shards is not None:
+            return self._add_memory_sharded(image, pix_feat, prob, key, shrinkage, selection, ids,
+                                            is_deep_update=is_deep_update, force_permanent=force_permanent)
         self.memory.initialize_sensory_if_needed(key, ids)
         graphed = (self.use_cuda_graphs and self._graphs is not None and _graphable(image) and is_deep_update and
                    not self.flip_aug and self.chunk_size < 1 and not self.save_aux and
@@ -201,6 +220,26 @@ class InferenceCore:
         self.last_mem_ti = self.curr_ti
         if is_deep_update:
             self.memory.update_sensory(sensory, ids)
+
+    def _add_memory_sharded(self, image, pix_feat, prob, key, shrinkage, selection, ids, *, is_deep_update: bool,
+                            force_permanent: bool) -> None:
+        """_add_memory under object sharding: the mask encoder and summarizer run on this rank's objects (the others-mask
+        from all of `prob`); keys go to memory on every rank, values only on the owner's."""
+        grp = self.object_shards.group_of(ids)
+        local = grp.local_ids
+        self.memory.initialize_sensory_if_needed(key, local)
+        if local:
+            msk_value, sensory, obj_value, _ = self.network.encode_mask(
+                image, pix_feat, self.memory.get_sensory(local), prob, deep_update=is_deep_update,
+                chunk_size=self.chunk_size, objects=grp)
+        else:
+            msk_value = key.new_empty(key.shape[0], 0, self.network.value_dim, *key.shape[-2:])
+            sensory = obj_value = None
+        self.memory.add_memory(key, shrinkage, msk_value, obj_value, ids, selection=selection,
+                               as_permanent='all' if force_permanent else 'first')
+        self.last_mem_ti = self.curr_ti
+        if is_deep_update and local:
+            self.memory.update_sensory(sensory, local)
 
     def _segment(self, key, selection, pix_feat, ms_features: Iterable[torch.Tensor],
                  update_sensory: bool = True) -> torch.Tensor:
@@ -226,6 +265,16 @@ class InferenceCore:
             logits, prob = logits.clone(), prob.clone()
             if update_sensory:
                 sensory = sensory.clone()
+        elif self.object_shards is not None:
+            readout = self.memory.read(pix_feat, key, selection, self.last_mask, self.network)
+            grp = self.object_shards.group_of(ids)
+            ids = grp.local_ids
+            readout = torch.stack([readout[o] for o in ids], dim=1) if ids else None
+            sensory, logits, prob = self.network.segment(ms_features, readout,
+                                                         self.memory.get_sensory(ids) if ids else None,
+                                                         chunk_size=self.chunk_size, update_sensory=update_sensory,
+                                                         objects=grp)
+            update_sensory = update_sensory and bool(ids)
         else:
             readout = self.memory.read(pix_feat, key, selection, self.last_mask, self.network)
             readout = self.object_manager.realize_dict(readout)
@@ -241,7 +290,7 @@ class InferenceCore:
         return prob
 
     def _graph_path_ok(self, key: torch.Tensor, ids) -> bool:
-        if not (self.use_cuda_graphs and _graphable(key)):
+        if not (self.use_cuda_graphs and _graphable(key)) or self.object_shards is not None:
             return False
         m = self.memory
         if self.flip_aug or self.chunk_size >= 1 or self.save_aux or len(m.work_mem.buckets) != 1:
@@ -329,12 +378,18 @@ class InferenceCore:
         else:
             ms_feat, pix_feat = self.image_feature_store.get_features(self.curr_ti, image)
             key, shrinkage, selection = self.image_feature_store.get_key(self.curr_ti, image)
+        if self.object_shards is not None:
+            # every rank's top-k, usage and memory keys follow rank 0's keys: the replicated state stays identical even
+            # where a library call (e.g. an autotuned cuDNN convolution of the encoder) rounds differently on some rank
+            key, shrinkage, selection = self.object_shards.broadcast((key, shrinkage, selection))
 
         if need_segment:
             prob_with_bg = self._segment(key, selection, pix_feat, ms_feat, update_sensory=update_sensory)
 
         if mask is not None:
             tmp_ids, _ = self.object_manager.add_new_objects(objects)
+            if self.object_shards is not None:
+                self.object_shards.add(self.object_manager.all_obj_ids)
             mask, _ = pad_divide_by(mask, 16)
             if need_segment:
                 # merge the propagated prediction with the (partial) input mask; input wins where it is set
@@ -391,6 +446,8 @@ class InferenceCore:
     def delete_objects(self, objects: List[int]) -> None:
         self.object_manager.delete_objects(objects)
         self.memory.purge_except(self.object_manager.all_obj_ids)
+        if self.object_shards is not None:
+            self.object_shards.retain(self.object_manager.all_obj_ids)
 
     def output_prob_to_mask(self, output_prob: torch.Tensor) -> torch.Tensor:
         """argmax over channels, then tmp-id -> object-id remap (one fused kernel on the GPU)."""

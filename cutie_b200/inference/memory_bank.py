@@ -181,6 +181,8 @@ class KeyValueMemoryStore:
         self._objs: Dict[int, int] = {}          # object id -> bucket id
         self.temp_hint = 0                       # capacity hints (tokens) applied to every bucket's arenas
         self.perm_hint = 0
+        # object sharding: value arrays are kept only for the objects this predicate accepts (keys for all of them)
+        self.keeps_values = None
 
     # -- reference surface: sizes ----------------------------------------------------------
     @property
@@ -223,7 +225,8 @@ class KeyValueMemoryStore:
                 arena.declare('use', 0, B, device)
                 arena.declare('life', 0, B, device)
             for o in objs:
-                arena.declare(('val', o), CV, B, device)
+                if self.keeps_values is None or self.keeps_values(o):
+                    arena.declare(('val', o), CV, B, device)
 
     def slots_for_add(self, obj_ids: List[int], ne: int, B: int, CK: int, CV: int, device,
                       supposed_bucket_id: int = -1,
@@ -282,13 +285,14 @@ class KeyValueMemoryStore:
 
     def add(self, key: torch.Tensor, values: Dict[int, torch.Tensor], shrinkage: torch.Tensor,
             selection: Optional[torch.Tensor], supposed_bucket_id: int = -1,
-            as_permanent: Literal['no', 'first', 'all'] = 'no') -> None:
+            as_permanent: Literal['no', 'first', 'all'] = 'no', *, objects: Optional[List[int]] = None) -> None:
         """Reference-shaped insert: key [B,CK,n], values {obj: [B,CV,n]}, shrinkage [B,1,n],
-        selection [B,CK,n] (channel-major, as the encoders emit them)."""
+        selection [B,CK,n] (channel-major, as the encoders emit them).  objects (object sharding): all objects of the
+        frame, which place the tokens in buckets; `values` then holds those whose values this store keeps."""
         B, CK, ne = key.shape
         assert shrinkage.dim() == 3 and (not self.save_selection or selection.dim() == 3)
-        objs = list(values.keys())
-        CV = values[objs[0]].shape[1]
+        objs = list(values.keys()) if objects is None else list(objects)
+        CV = next(iter(values.values())).shape[1] if values else 0
         for b, arena, runs, permanent in self.slots_for_add(objs, ne, B, CK, CV, key.device,
                                                             supposed_bucket_id, as_permanent):
             pos = 0
@@ -466,7 +470,8 @@ class KeyValueMemoryStore:
 
     @property
     def value(self) -> Dict[int, torch.Tensor]:
-        return {o: self._export(b, ('val', o), True) for o, b in self._objs.items()}
+        return {o: self._export(b, ('val', o), True) for o, b in self._objs.items()
+                if ('val', o) in self._b[b].temp.widths}
 
     # reference attribute aliases (memory_manager / GUI code reads .k/.v/.s/.e in places)
     k, v, s, e = key, value, shrinkage, selection

@@ -71,14 +71,19 @@ def _neighbour_offsets(n: int, width: int, frame_tokens: int, device) -> torch.T
 
 
 class MemoryManager:
-    def __init__(self, cfg, object_manager: ObjectManager, *, shard_group=None):
+    def __init__(self, cfg, object_manager: ObjectManager, *, shard_group=None, object_shards=None):
         """shard_group (a torch.distributed process group, or None): key-shard THIS stream's memory over the group's
         ranks (SURVEY.md 8(e).2).  Every rank runs the same frames through the same model; each stores the slice
         shard_bounds(HW, world, rank) of every memory frame's tokens and the read exchanges top-k candidates
         (all_gather) and partial readouts (all_reduce) -- cutie_b200/inference/sharded.py.  With use_long_term the
         long-term store is sharded too: prototypes are chosen by a global usage ranking, potentiated shard-wise (all_gather
-        of the per-shard affinity maxima and exp-sums) and dealt to the ranks in contiguous blocks of that ranking."""
+        of the per-shard affinity maxima and exp-sums) and dealt to the ranks in contiguous blocks of that ranking.
+
+        object_shards (an object_shards.ObjectShards, or None): keys, shrinkage, selections, top-k, usage and long-term
+        maintenance are kept for every object on every rank (the same decisions everywhere); value arrays, sensory
+        state and object summaries only for the objects this rank owns.  read() then returns this rank's objects."""
         self.object_manager = object_manager
+        self.object_shards = object_shards
         self.shard_group = shard_group
         self.shard_world, self.shard_rank = 1, 0
         if shard_group is not None:
@@ -104,6 +109,11 @@ class MemoryManager:
         if self.use_long_term:
             self.long_mem = KeyValueMemoryStore(save_usage=self.count_long_term_usage, ring=False,
                                                 key_centres=self.work_mem.key_centres)
+        if object_shards is not None:
+            owns = lambda o: object_shards.owner[o] == object_shards.rank          # noqa: E731
+            self.work_mem.keeps_values = owns
+            if self.use_long_term:
+                self.long_mem.keeps_values = owns
         self.config_stale = True
         self.engaged = False
         self.aux = None
@@ -132,6 +142,11 @@ class MemoryManager:
         self._read_sizes(cfg)
 
     # -- helpers -----------------------------------------------------------------------------
+    def local_ids(self, obj_ids: List[int]) -> List[int]:
+        """The objects of `obj_ids` whose values / sensory / summaries this manager holds (object sharding: the ones
+        this rank owns), in the order of `obj_ids`."""
+        return list(obj_ids) if self.object_shards is None else self.object_shards.local(obj_ids)
+
     def _get_mask_by_ids(self, mask: torch.Tensor, obj_ids: List[int]) -> torch.Tensor:
         return mask[:, [self.object_manager.find_tmp_by_id(o) - 1 for o in obj_ids]]
 
@@ -229,6 +244,23 @@ class MemoryManager:
         for bucket_id, bucket in self.work_mem.buckets.items():
             gather = self._topk(bucket_id, qk, qe)
 
+            if self.object_shards is not None:       # chunk_size < 1, save_aux off (InferenceCore checks)
+                grp = self.object_shards.group_of(bucket)
+                objects = grp.local_ids
+                if not objects:
+                    if getattr(network, 'object_transformer_enabled', True):
+                        network.object_transformer.exchange_without_objects(grp, bs, h * w, pix_feat.device)
+                    continue
+                visual = gather(objects).view(bs, len(objects), self.CV, h, w)
+                pixel_readout = network.pixel_fusion(pix_feat, visual, self._get_sensory_by_ids(objects),
+                                                     self._get_mask_by_ids(last_mask, bucket), objects=grp)
+                obj_mem = self._get_object_mem_by_ids(objects)
+                obj_mem = obj_mem.unsqueeze(2) if obj_mem is not None else None
+                readout_memory, _ = network.readout_query(pixel_readout, obj_mem, objects=grp)
+                for i, o in enumerate(objects):
+                    out[o] = readout_memory[:, i]
+                continue
+
             if self.chunk_size < 1:
                 chunks = [bucket]
             else:
@@ -271,7 +303,8 @@ class MemoryManager:
     def add_memory(self, key: torch.Tensor, shrinkage: torch.Tensor, msk_value: torch.Tensor,
                    obj_value: Optional[torch.Tensor], objects: List[int],
                    selection: Optional[torch.Tensor] = None, *, as_permanent='no') -> None:
-        """key [B,CK,h,w]; shrinkage [B,1,h,w]; msk_value [B,K,CV,h,w]; obj_value [B,K,Q,E+1]."""
+        """key [B,CK,h,w]; shrinkage [B,1,h,w]; msk_value [B,K,CV,h,w]; obj_value [B,K,Q,E+1].
+        Object sharding: `objects` are all objects of the frame, msk_value / obj_value hold local_ids(objects)."""
         bs = key.shape[0]
         assert shrinkage.shape[0] == bs
         assert msk_value.shape[0] == bs
@@ -280,7 +313,7 @@ class MemoryManager:
         self.engaged = True
         if self.H is None or self.config_stale:
             self.config_stale = False
-            self.H, self.W = msk_value.shape[-2:]
+            self.H, self.W = key.shape[-2:]
             self.HW = self.HW_global = self.H * self.W
             if self.shard_group is not None:              # sizes below are in LOCAL tokens (this rank's slice)
                 from cutie_b200.inference.sharded import shard_bounds
@@ -306,16 +339,18 @@ class MemoryManager:
             key, shrinkage, msk_value = key[:, :, sl], shrinkage[:, :, sl], msk_value[:, :, :, sl]
             selection = selection[:, :, sl] if selection is not None else None
 
+        local = self.local_ids(objects)
         if obj_value is not None:                       # streaming sums (memory_manager.py:252-271)
-            for i, obj in enumerate(objects):
+            for i, obj in enumerate(local):
                 new = obj_value[:, i].contiguous()
                 if obj in self.obj_v:
                     K_.obj_summary_accumulate(self.obj_v[obj], new)
                 else:
                     self.obj_v[obj] = new.clone()
 
-        values = {obj: msk_value[:, i] for i, obj in enumerate(objects)}
-        self.work_mem.add(key, values, shrinkage, selection=selection, as_permanent=as_permanent)
+        values = {obj: msk_value[:, i] for i, obj in enumerate(local)}
+        self.work_mem.add(key, values, shrinkage, selection=selection, as_permanent=as_permanent,
+                          objects=objects if self.object_shards is not None else None)
 
         for bucket_id in self.work_mem.buckets.keys():
             if self.use_long_term:
@@ -359,6 +394,7 @@ class MemoryManager:
         if self.shard_group is not None:
             return self._consolidation_sharded(bucket_id, n_cand)
         objs = self.work_mem.buckets[bucket_id]
+        vobjs = self.local_ids(objs)
         arena, runs = self.work_mem.temp_runs(bucket_id, 0, n_cand)
         bs = arena.B
         dev = arena.device
@@ -372,9 +408,9 @@ class MemoryManager:
         K_.bank_gather([arena.view('key', r) for r in runs], proto_idx, larena.view('key', lrun))
         proto_sel = torch.empty(bs, P, self.CK, dtype=torch.float32, device=dev)
         K_.bank_gather([arena.view('sel', r) for r in runs], proto_idx, proto_sel)
-        cand = self.work_mem.segments(bucket_id, objs, perm=False, temp_start=0, temp_len=n_cand)
+        cand = self.work_mem.segments(bucket_id, vobjs, perm=False, temp_start=0, temp_len=n_cand)
         K_.consolidate(cand, larena.view('key', lrun), proto_sel,
-                       [larena.view(('val', o), lrun) for o in objs], larena.view('shr', lrun))
+                       [larena.view(('val', o), lrun) for o in vobjs], larena.view('shr', lrun))
 
     # -- the same, key-sharded (cutie_b200/inference/sharded.py) ---------------------------------------
     def _consolidation_sharded(self, bucket_id: int, n_cand: int) -> None:

@@ -803,6 +803,33 @@ def qt_aux_mask(pixel: torch.Tensor, w: torch.Tensor, b: torch.Tensor, B: int, K
     return logits, fg, cnt
 
 
+def qt_mask_logits(pixel: torch.Tensor, w: torch.Tensor, b: torch.Tensor, B: int, K: int) -> torch.Tensor:
+    """The first half of qt_aux_mask: mask_pred's logits alone, pixel [B*K, E, HW] -> f32 [B,K,HW], the same bits."""
+    BK, E, HW = pixel.shape
+    assert pixel.is_contiguous(), 'pixel must be channel-major contiguous [B*K, E, HW]'
+    logits = torch.empty(B, K, HW, dtype=torch.float32, device=pixel.device)
+    with _call('qt_mask_logits', 1):
+        st = lib().cutie_qt_mask_logits(_ptr(pixel), _ptr(w), _ptr(b), _i64(B), _i64(K), _i64(E), _i64(HW),
+                                        _ptr(logits), _stream())
+    _check(st, 'cutie_qt_mask_logits')
+    return logits
+
+
+def qt_aux_fg(logits: torch.Tensor, positions: torch.Tensor):
+    """The second half of qt_aux_mask: logits f32 [B,K,HW] of ALL objects, positions int32 [n] (CUDA; entries in [0, K))
+    -> (fg uint8 [B,n,HW], fg_count int32 [B*n]) of the objects at those positions, the bits qt_aux_mask gives them."""
+    B, K, HW = logits.shape
+    n = positions.numel()
+    assert logits.is_contiguous() and positions.is_contiguous()
+    fg = torch.empty(B, n, HW, dtype=torch.uint8, device=logits.device)
+    cnt = torch.zeros(B * n, dtype=torch.int32, device=logits.device)
+    with _call('qt_aux_fg', 1):
+        st = lib().cutie_qt_aux_fg(_ptr(logits), _ptr(positions, torch.int32), _i64(B), _i64(K), _i64(n), _i64(HW),
+                                   _ptr(fg, torch.uint8), _ptr(cnt, torch.int32), _stream())
+    _check(st, 'cutie_qt_aux_fg')
+    return fg, cnt
+
+
 def qt_pixel_to_query_tiles(qfold: torch.Tensor, pixel: torch.Tensor, pixel_pe: torch.Tensor, fg: torch.Tensor,
                             fg_count: torch.Tensor, num_queries: int, num_heads: int = 8):
     """The tensor-core half of qt_pixel_to_query only: per 64-pixel tile and object the tile-local softmax statistics and

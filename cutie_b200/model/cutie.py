@@ -22,6 +22,11 @@ from cutie_b200.utils.tensor_utils import aggregate
 log = logging.getLogger()
 
 
+def _local(x: Optional[torch.Tensor], objects) -> Optional[torch.Tensor]:
+    """The rows of this rank's objects of `objects` (object_shards.ObjectGroup) along the object axis (dim 1)."""
+    return None if x is None else x[:, objects.positions]
+
+
 class _SensoryAuxHead(nn.Module):
     """Training-time auxiliary head (cutie/model/aux_modules.py:14-27); kept so checkpoints load 1:1."""
 
@@ -99,9 +104,14 @@ class CUTIE(nn.Module):
         return self.key_proj(final_pix_feat, need_s=need_sk, need_e=need_ek)
 
     def encode_mask(self, image, ms_features, sensory, masks, *, deep_update: bool = True,
-                    chunk_size: int = -1, need_weights: bool = False):
+                    chunk_size: int = -1, need_weights: bool = False, objects=None):
+        """objects (extension; object sharding): an object_shards.ObjectGroup over the objects of `masks`; `sensory`
+        and the results are this rank's objects of it, the others-mask is formed from all of `masks`."""
+        others = self._others(masks)
+        if objects is not None:
+            masks, others = _local(masks, objects), _local(others, objects)
         value, new_sensory = self.mask_encoder(self._normalise(image), ms_features, sensory, masks,
-                                               self._others(masks), deep_update=deep_update,
+                                               others, deep_update=deep_update,
                                                chunk_size=chunk_size)
         if self.object_transformer_enabled:
             summaries, logits = self.object_summarizer(masks, value, need_weights)
@@ -110,17 +120,21 @@ class CUTIE(nn.Module):
         return value, new_sensory, summaries, logits
 
     # -- hot path, model side --------------------------------------------------------------
-    def pixel_fusion(self, pix_feat, pixel, sensory, last_mask, *, chunk_size: int = -1):
-        """cutie.py:142-157 (a8)."""
+    def pixel_fusion(self, pix_feat, pixel, sensory, last_mask, *, chunk_size: int = -1, objects=None):
+        """cutie.py:142-157 (a8).  objects (extension; object sharding): an object_shards.ObjectGroup over the objects
+        of `last_mask`; `pixel`, `sensory` and the result are this rank's objects of it."""
         last_mask = area_resize(self, last_mask, sensory.shape[-2:])
-        return self.pixel_fuser(pix_feat, pixel, sensory, last_mask, self._others(last_mask),
-                                chunk_size=chunk_size)
+        others = self._others(last_mask)
+        if objects is not None:
+            last_mask, others = _local(last_mask, objects), _local(others, objects)
+        return self.pixel_fuser(pix_feat, pixel, sensory, last_mask, others, chunk_size=chunk_size)
 
-    def readout_query(self, pixel_readout, obj_memory, *, selector=None, need_weights: bool = False):
-        """cutie.py:159-170 (a9)."""
+    def readout_query(self, pixel_readout, obj_memory, *, selector=None, need_weights: bool = False, objects=None):
+        """cutie.py:159-170 (a9).  objects (extension; object sharding): see QueryTransformer.forward."""
         if not self.object_transformer_enabled:
             return pixel_readout, None
-        return self.object_transformer(pixel_readout, obj_memory, selector=selector, need_weights=need_weights)
+        return self.object_transformer(pixel_readout, obj_memory, selector=selector, need_weights=need_weights,
+                                       objects=objects)
 
     def read_memory(self, *args, **kwargs):
         """Training-time dense read (cutie.py:102-140): outside the inference hot path."""
@@ -128,11 +142,18 @@ class CUTIE(nn.Module):
 
     # -- stage after the hot path ----------------------------------------------------------
     def segment(self, ms_image_feat: List[torch.Tensor], memory_readout, sensory, *, selector=None,
-                chunk_size: int = -1, update_sensory: bool = True):
-        """cutie.py:172-203 -> (sensory, logits [B,1+K,16h,16w], prob)."""
-        sensory, logits = self.mask_decoder(ms_image_feat, memory_readout, sensory, chunk_size=chunk_size,
-                                            update_sensory=update_sensory)
-        raw = logits
+                chunk_size: int = -1, update_sensory: bool = True, objects=None):
+        """cutie.py:172-203 -> (sensory, logits [B,1+K,16h,16w], prob).
+        objects (extension; object sharding): an object_shards.ObjectGroup over all objects.  `memory_readout` and
+        `sensory` hold this rank's objects of it (None if it owns none) and so does the returned sensory; the decoder
+        logits are all-gathered before the aggregation, so `logits` and `prob` cover every object."""
+        if objects is not None and not objects.local_ids:
+            f16 = ms_image_feat[0]
+            sensory, logits = None, f16.new_empty(f16.shape[0], 0, 4 * f16.shape[-2], 4 * f16.shape[-1])
+        else:
+            sensory, logits = self.mask_decoder(ms_image_feat, memory_readout, sensory, chunk_size=chunk_size,
+                                                update_sensory=update_sensory)
+        raw = logits if objects is None else objects.gather(logits)
 
         def aten():
             prob = torch.sigmoid(raw)

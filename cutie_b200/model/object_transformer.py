@@ -158,15 +158,30 @@ class QueryTransformer(nn.Module):
         self.mask_pred = nn.ModuleList(nn.Sequential(nn.ReLU(), ObjConv2d(E, 1, 1))
                                        for _ in range(self.num_blocks + 1))
 
-    def _aux(self, i: int, pixel_cm: torch.Tensor, B: int, K: int):
+    def _aux(self, i: int, pixel_cm: torch.Tensor, B: int, K: int, objects=None):
+        """mask_pred[i] + the foreground test.  With `objects` (an object_shards.ObjectGroup: `pixel_cm` holds its
+        local objects) the test runs against the logits of all the group's objects, all-gathered from their owners.
+        forward() calls this once per head of mask_pred, in order: exchange_without_objects relies on it."""
         conv = self.mask_pred[i][1]
-        return K_.qt_aux_mask(pixel_cm, conv.weight.view(-1), conv.bias, B, K)
+        if objects is None:
+            return K_.qt_aux_mask(pixel_cm, conv.weight.view(-1), conv.bias, B, K)
+        logits = K_.qt_mask_logits(pixel_cm, conv.weight.view(-1), conv.bias, B, K)
+        fg, cnt = K_.qt_aux_fg(objects.gather(logits), objects.positions_tensor(logits.device))
+        return logits, fg, cnt
+
+    def exchange_without_objects(self, objects, B: int, hw: int, device) -> None:
+        """A rank that owns none of `objects` joins the all-gather of every _aux call forward() makes (one per head of
+        mask_pred), contributing no rows, so that the ranks' collectives stay in step."""
+        for _ in self.mask_pred:
+            objects.gather(torch.empty(B, 0, hw, device=device))
 
     def forward(self, pixel: torch.Tensor, obj_summaries: torch.Tensor, selector: Optional[torch.Tensor] = None,
-                need_weights: bool = False):
+                need_weights: bool = False, *, objects=None):
         """pixel [B,K,E,h,w]; obj_summaries [B,K,T,Q,E+1] -> (pixel [B,K,E,h,w], aux dict)
         (object_transformer.py:114-177).  `selector` (training-time object padding) and `need_weights`
-        (attention-map export) are not part of the inference hot path and are rejected."""
+        (attention-map export) are not part of the inference hot path and are rejected.
+        objects (extension; object sharding): the object_shards.ObjectGroup of the objects whose foreground tests
+        couple; `pixel` holds this rank's objects of it."""
         if selector is not None or need_weights or self.training:
             raise NotImplementedError('cutie_b200 implements the inference path (selector=None, need_weights=False)')
         B, K, E, h, w = pixel.shape
@@ -175,7 +190,7 @@ class QueryTransformer(nn.Module):
             obj_summaries = obj_summaries.sum(dim=2, keepdim=True)      # sums and areas both add (:128-131)
         summ = obj_summaries.reshape(B * K * Q, E + 1).contiguous()
         if QT_CHAIN and (h * w + 63) // 64 <= K_.QT_CHAIN_MAX_TILES:
-            return self._forward_chained(pixel, summ)
+            return self._forward_chained(pixel, summ, objects)
         x = K_.qt_linear(summ, self.summary_to_query_init.weight, self.summary_to_query_init.bias,
                          summary_norm=True, residual=self.query_init.weight, residual_mod=Q)
         query_pe = K_.qt_linear(summ, self.summary_to_query_emb.weight, self.summary_to_query_emb.bias,
@@ -186,11 +201,12 @@ class QueryTransformer(nn.Module):
         pe = self.spatial_pe.grid(h, w).reshape(h * w, E).t()                     # [E, HW]
         pixel_pe = (self.pixel_emb_proj(pixel).reshape(B * K, E, h * w) + pe).contiguous()
 
-        logits, fg, cnt = self._aux(0, pix, B, K)
+        # one _aux call per head of mask_pred (exchange_without_objects mirrors these under object sharding)
+        logits, fg, cnt = self._aux(0, pix, B, K, objects)
         aux_logits = [logits.view(B, K, h, w)]
         for i, blk in enumerate(self.blocks):
             x, pix = blk(x, pix, query_pe, pixel_pe, fg, cnt, (h, w))
-            logits, fg, cnt = self._aux(i + 1, pix, B, K)                          # :164-167 (always taken)
+            logits, fg, cnt = self._aux(i + 1, pix, B, K, objects)                 # :164-167 (always taken)
             aux_logits.append(logits.view(B, K, h, w))
         return self._finish(pix, aux_logits, fg, B, K, E, h, w)
 
@@ -199,7 +215,7 @@ class QueryTransformer(nn.Module):
                                   'fg_map': fg.view(B, K, h, w)}
         return pix.view(B, K, E, h, w), aux
 
-    def _forward_chained(self, pixel: torch.Tensor, summ: torch.Tensor):
+    def _forward_chained(self, pixel: torch.Tensor, summ: torch.Tensor, objects=None):
         """forward() with the query-side ops fused: one cutie_qt_chain launch for the query initialisation and block 0's
         query projection, then per block [read_from_pixel tiles on wgmma] -> ONE chain (merge + value projection,
         out-proj, self attention, FFN, this block's key/value folds and the NEXT block's query fold) -> [read_from_query on
@@ -231,7 +247,8 @@ class QueryTransformer(nn.Module):
         pix = self.pixel_init_proj(pixel).reshape(BK, E, h * w).contiguous()
         pe = self.spatial_pe.grid(h, w).reshape(h * w, E).t()                     # [E, HW]
         pixel_pe = (self.pixel_emb_proj(pixel).reshape(BK, E, h * w) + pe).contiguous()
-        logits, fg, cnt = self._aux(0, pix, B, K)
+        # one _aux call per head of mask_pred (exchange_without_objects mirrors these under object sharding)
+        logits, fg, cnt = self._aux(0, pix, B, K, objects)
         aux_logits = [logits.view(B, K, h, w)]
         for i, blk in enumerate(self.blocks):
             rp, sa, f, rq = blk.read_from_pixel, blk.self_attn, blk.ffn, blk.read_from_query
@@ -271,7 +288,7 @@ class QueryTransformer(nn.Module):
             ch.run()
             pix = K_.qt_query_to_pixel(kfold, kdots, vfold, rq.cross_attn.out_proj.bias, pix, pixel_pe, Q, H)
             pix = blk.pixel_ffn.conv(pix.view(BK, E, h, w)).reshape(BK, E, -1).contiguous()
-            logits, fg, cnt = self._aux(i + 1, pix, B, K)                          # :164-167 (always taken)
+            logits, fg, cnt = self._aux(i + 1, pix, B, K, objects)                 # :164-167 (always taken)
             aux_logits.append(logits.view(B, K, h, w))
         return self._finish(pix, aux_logits, fg, B, K, E, h, w)
 

@@ -31,6 +31,9 @@
 extern "C" {
 #endif
 
+/* The version changes when an existing entry point changes its signature or meaning.  Adding entry points leaves it
+ * alone: a caller built against an older header finds every symbol it knew, unchanged (cutie_qt_mask_logits and
+ * cutie_qt_aux_fg were added at version 1). */
 #define CUTIE_B200_ABI_VERSION 1
 #define CUTIE_B200_MAX_SEGMENTS 4       /* long | permanent | ring piece a | ring piece b */
 #define CUTIE_B200_USAGE_FRAC_BITS 40   /* usage accumulators: uint64 fixed point, 2^-40 */
@@ -328,6 +331,17 @@ int cutie_qt_chain(const cutie_qt_op* ops, int nops, const void* const* prefetch
  * above 32 objects a streaming form runs the same floating-point operations in the same order. */
 int cutie_qt_aux_mask(const float* pixel, const float* w, const float* b, int64_t B, int64_t K, int64_t E,
                       int64_t HW, float* logits, uint8_t* fg, int32_t* fg_count, void* stream);
+/* cutie_qt_aux_mask in two halves, for objects split over ranks (object sharding): every rank computes the logits of its
+ * own objects, the ranks exchange them, and each runs the foreground test of its objects against all K.  Together they
+ * give the same bits as cutie_qt_aux_mask.
+ * cutie_qt_mask_logits: the mask_pred 1x1 conv on relu(pixel) alone, pixel [B*K, E, HW] -> logits [B, K, HW].
+ * cutie_qt_aux_fg: logits [B, K, HW] of ALL objects; positions int32 [n] (device, each in [0, K), any order, e.g. the
+ * tmp-id positions of one rank's objects) -> fg uint8 [B, n, HW] and fg_count int32 [B*n] (zeroed by the caller) of the
+ * objects at those positions.  Up to 32 objects a pixel's logits stay in registers, above they are streamed. */
+int cutie_qt_mask_logits(const float* pixel, const float* w, const float* b, int64_t B, int64_t K, int64_t E,
+                         int64_t HW, float* logits, void* stream);
+int cutie_qt_aux_fg(const float* logits, const int32_t* positions, int64_t B, int64_t K, int64_t n, int64_t HW,
+                    uint8_t* fg, int32_t* fg_count, void* stream);
 /* read_from_pixel attention core (masked, queries <- pixels) on the tensor cores (wgmma) (3xTF32, fp32-class accuracy):
  * one CTA per 64-pixel tile and object computes S = Qfold.(pixel+pe), the masked tile-local softmax and Z = P.pixel^T
  * (csrc/qt_tc.cu); a combine kernel merges the tiles and applies the per-head value projection.  Replaces
