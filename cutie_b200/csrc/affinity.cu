@@ -723,11 +723,10 @@ extern "C" size_t cutie_affinity_workspace_bytes(int64_t B, int64_t Q, int64_t n
   return ws_layout(B, Q, n_total, top_k).total;
 }
 
-// Banks with fewer tokens than this use the exact scan only (default 8192; env CUTIE_B200_TC_MIN /
+// Banks with fewer tokens than this use the exact scan only (default 6144; env CUTIE_B200_TC_MIN /
 // CUTIE_B200_NO_TC=1).  Negative restores the default.  Process-wide; meant for tests and tuning.
 extern "C" void cutie_set_tc_min_tokens(int64_t n) { g_tc_min_override = n; }
 
-// Which plan cutie_affinity_topk will use: 1 = exact scan only, 2/3 = wgmma filter levels (see make_plan).
 // Per-phase device times (ms) of a filtered cutie_affinity_topk call: filter level, threshold select, ..., re-rank.
 // cutie_debug_phase_timing(1) starts recording (a ring of the last 64 calls); cutie_debug_phase_times(calls_ago, ...)
 // waits for that call's last event and returns the number of phases written.
@@ -747,6 +746,7 @@ extern "C" int cutie_debug_phase_times(int64_t calls_ago, float* out_ms, int max
 // How many filter levels have been served from a key image so far in this process (diagnostics / tests).
 extern "C" int64_t cutie_debug_image_level_launches(void) { return g_image_level_launches; }
 
+// Which plan cutie_affinity_topk will use: 0 = exact scan only, n >= 1 = n wgmma filter levels (see make_plan).
 extern "C" int cutie_affinity_plan_levels(int64_t n_total, int top_k) { return make_plan(n_total, top_k).levels; }
 
 // Diagnostics: byte offset of the per-query candidate counters [B][Q] int32 inside the workspace (-1: exact-scan plan).
@@ -758,21 +758,16 @@ extern "C" int64_t cutie_debug_ws_count_offset(int64_t B, int64_t Q, int64_t n_t
 static int fill_scan_params(ScanParams& sp, int num_segments, const void* const* seg_key,
                             const void* const* seg_shrinkage, const int64_t* seg_len,
                             const int64_t* seg_key_bstride, const int64_t* seg_shr_bstride, const float* qk,
-                            const float* qe, int64_t Q, int top_k, int kpad, int64_t n_total) {
+                            const float* qe, int64_t Q, int top_k, int kpad, int64_t n_total, const char* fn) {
   memset(&sp, 0, sizeof(sp));
-  long long tot = 0;
+  if (int rc = segment_table(sp.segs.begin, num_segments, seg_len, &n_total, fn)) return rc;
   for (int s = 0; s < num_segments; ++s) {
-    if (seg_len[s] < 0) return fail(-1, "%s: negative segment length", "cutie_affinity_topk");
     sp.segs.key[s] = (const float*)seg_key[s];
     sp.segs.shr[s] = (const float*)seg_shrinkage[s];
     sp.segs.key_bs[s] = seg_key_bstride[s];
     sp.segs.shr_bs[s] = seg_shr_bstride[s];
-    sp.segs.begin[s] = tot;
-    tot += seg_len[s];
   }
-  for (int s = num_segments; s <= kMaxSeg; ++s) sp.segs.begin[s] = tot;
   sp.segs.nseg = num_segments;
-  if (tot != n_total) return fail(-1, "%s: n_total != sum of segment lengths", "cutie_affinity_topk");
   sp.qk = qk;
   sp.qe = qe;
   sp.Q = Q;
@@ -794,7 +789,6 @@ extern "C" int cutie_affinity_topk_img(int num_segments, const void* const* seg_
                                        int64_t CK, int64_t Q, int top_k, int kpad, int32_t* out_idx, float* out_w,
                                        float* out_sim, unsigned long long* usage_acc, int64_t n_total,
                                        void* workspace, size_t workspace_bytes, void* stream) {
-  CUTIE_REQUIRE(num_segments >= 1 && num_segments <= kMaxSeg, "1..4 segments");
   CUTIE_REQUIRE(CK == CKD, "CK must be 64");
   CUTIE_REQUIRE(kpad == 32 || kpad == 64, "kpad must be 32 or 64");
   CUTIE_REQUIRE(top_k >= 1 && top_k <= kpad, "1 <= top_k <= kpad");
@@ -803,7 +797,7 @@ extern "C" int cutie_affinity_topk_img(int num_segments, const void* const* seg_
   CUTIE_REQUIRE(n_total < (1ll << 31), "bank too large for int32 indices");
   ScanParams sp;
   int rc = fill_scan_params(sp, num_segments, seg_key, seg_shrinkage, seg_len, seg_key_bstride, seg_shr_bstride, qk,
-                            qe, Q, top_k, kpad, n_total);
+                            qe, Q, top_k, kpad, n_total, __func__);
   if (rc) return rc;
   const WsLayout wl = ws_layout(B, Q, n_total, top_k);
   CUTIE_REQUIRE(workspace_bytes >= wl.total, "workspace too small");
@@ -855,11 +849,11 @@ extern "C" int cutie_debug_tc_energy(int num_segments, const void* const* seg_ke
                                      const int64_t* seg_shr_bstride, const float* qk, const float* qe, int64_t B,
                                      int64_t Q, int64_t n_total, float* dbg_energy, void* workspace,
                                      size_t workspace_bytes, void* stream) {
-  CUTIE_REQUIRE(num_segments >= 1 && num_segments <= kMaxSeg && dbg_energy && workspace, "bad argument");
+  CUTIE_REQUIRE(dbg_energy && workspace, "bad argument");
   CUTIE_REQUIRE(n_total <= TC_CAP, "debug hook handles at most 4096 tokens");
   ScanParams sp;
   int rc = fill_scan_params(sp, num_segments, seg_key, seg_shrinkage, seg_len, seg_key_bstride, seg_shr_bstride, qk,
-                            qe, Q, 1, 32, n_total);
+                            qe, Q, 1, 32, n_total, __func__);
   if (rc) return rc;
   WsLayout wl;
   memset(&wl, 0, sizeof(wl));
@@ -913,11 +907,12 @@ extern "C" int cutie_topk_merge(const float* part_val, const int32_t* part_idx, 
 extern "C" int cutie_readout_gather(const int32_t* idx, const float* w, int64_t B, int64_t Q, int kpad,
                                     int num_segments, const int64_t* seg_len, const void* const* seg_val,
                                     const int64_t* seg_val_bstride, int64_t K, int64_t CV, float* out, void* stream) {
-  CUTIE_REQUIRE(num_segments >= 1 && num_segments <= kMaxSeg, "1..4 segments");
   CUTIE_REQUIRE(CV == 256, "CV must be 256");
   CUTIE_REQUIRE(K >= 1, "at least one object");
   CUTIE_REQUIRE(kpad == 32 || kpad == 64, "kpad must be 32 or 64");
   CUTIE_REQUIRE(idx && w && out, "null argument");
+  long long begin[kMaxSeg + 1];
+  if (int rc = segment_table(begin, num_segments, seg_len, nullptr, __func__)) return rc;
   // The kernel's parameter block holds the row pointers of at most kMaxObj objects.  Each output plane out[b, k]
   // depends on object k alone, so larger calls launch once per group of kMaxObj objects with `out` offset by the
   // group; `K` stays the full count, the batch stride of `out`.
@@ -925,16 +920,12 @@ extern "C" int cutie_readout_gather(const int32_t* idx, const float* w, int64_t 
     const int nk = (int)(K - k0 < kMaxObj ? K - k0 : kMaxObj);
     GatherParams gp;
     memset(&gp, 0, sizeof(gp));
-    long long tot = 0;
-    for (int s = 0; s < num_segments; ++s) {
-      gp.segs.begin[s] = tot;
-      tot += seg_len[s];
+    memcpy(gp.segs.begin, begin, sizeof(begin));
+    for (int s = 0; s < num_segments; ++s)
       for (int k = 0; k < nk; ++k) {
         gp.segs.rows[s * nk + k] = (const float*)seg_val[s * K + k0 + k];
         gp.segs.bs[s * nk + k] = seg_val_bstride[s * K + k0 + k];
       }
-    }
-    for (int s = num_segments; s <= kMaxSeg; ++s) gp.segs.begin[s] = tot;
     gp.segs.nseg = num_segments;
     gp.segs.nobj = nk;
     gp.idx = idx;

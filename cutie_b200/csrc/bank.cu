@@ -264,19 +264,15 @@ extern "C" int cutie_bank_export(const float* rows, int64_t rows_bstride, float*
 extern "C" int cutie_bank_gather(int num_segments, const void* const* seg_rows, const int64_t* seg_len,
                                  const int64_t* seg_bstride, const int64_t* index, float* dst_rows,
                                  int64_t dst_bstride, int64_t B, int64_t m, int64_t C, void* stream) {
-  CUTIE_REQUIRE(num_segments >= 1 && num_segments <= kMaxSeg, "1..4 segments");
   CUTIE_REQUIRE(index && dst_rows && B >= 1 && C >= 1, "null/empty argument");
-  if (m <= 0) return 0;
   GatherRows g;
   memset(&g, 0, sizeof(g));
-  long long tot = 0;
+  if (int rc = segment_table(g.begin, num_segments, seg_len, nullptr, __func__)) return rc;
+  if (m <= 0) return 0;
   for (int s = 0; s < num_segments; ++s) {
     g.rows[s] = (const float*)seg_rows[s];
     g.bs[s] = seg_bstride[s];
-    g.begin[s] = tot;
-    tot += seg_len[s];
   }
-  for (int s = num_segments; s <= kMaxSeg; ++s) g.begin[s] = tot;
   g.nseg = num_segments;
   dim3 grid((unsigned)m, (unsigned)B);
   int threads = C >= 256 ? 256 : (C >= 64 ? 64 : 32);
@@ -295,25 +291,21 @@ extern "C" int cutie_consolidate_partial(int num_segments, const void* const* se
                                          float* out_max, float* out_sumexp, float* workspace, int64_t n_total,
                                          void* stream) {
   CUTIE_REQUIRE((out_max == nullptr) == (out_sumexp == nullptr), "out_max and out_sumexp come together");
-  CUTIE_REQUIRE(num_segments >= 1 && num_segments <= kMaxSeg, "1..4 segments");
   CUTIE_REQUIRE(CK == 64, "CK must be 64");
   CUTIE_REQUIRE(K >= 0, "negative object count");
   CUTIE_REQUIRE(K == 0 || CV == 256, "CV must be 256");
   CUTIE_REQUIRE(proto_key && proto_sel && out_shr && workspace && P >= 1 && B >= 1, "null/empty argument");
+  CUTIE_REQUIRE(n_total >= 1, "no candidate tokens");
   ConsParams cp;
   memset(&cp, 0, sizeof(cp));
-  long long tot = 0;
+  if (int rc = segment_table(cp.segs.begin, num_segments, seg_len, &n_total, __func__)) return rc;
+  memcpy(cp.vals.begin, cp.segs.begin, sizeof(cp.vals.begin));
   for (int s = 0; s < num_segments; ++s) {
     cp.segs.key[s] = (const float*)seg_key[s];
     cp.segs.shr[s] = (const float*)seg_shrinkage[s];
     cp.segs.key_bs[s] = seg_key_bstride[s];
     cp.segs.shr_bs[s] = seg_shr_bstride[s];
-    cp.segs.begin[s] = tot;
-    cp.vals.begin[s] = tot;
-    tot += seg_len[s];
   }
-  for (int s = num_segments; s <= kMaxSeg; ++s) cp.segs.begin[s] = cp.vals.begin[s] = tot;
-  CUTIE_REQUIRE(tot == n_total && n_total >= 1, "n_total != sum of segment lengths");
   cp.segs.nseg = cp.vals.nseg = num_segments;
   cp.pk = proto_key;
   cp.pk_bs = pk_bstride;

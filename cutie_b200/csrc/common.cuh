@@ -56,6 +56,25 @@ struct RowSegments {
   int nobj;
 };
 
+// The prefix table of a bank passed as (num_segments, seg_len[]): begin[s] = seg_len[0] + ... + seg_len[s-1], and every
+// entry from num_segments on holds the total, so seg_of() never steps past the last segment.  n_total (optional): the
+// total the caller was promised.  Returns 0, or -1 with `fn` in cutie_b200_last_error() for a segment count outside
+// 1..kMaxSeg, a negative length or lengths that do not sum to *n_total.
+inline int segment_table(long long (&begin)[kMaxSeg + 1], int num_segments, const int64_t* seg_len,
+                         const int64_t* n_total, const char* fn) {
+  if (num_segments < 1 || num_segments > kMaxSeg) return fail(-1, "%s: invalid argument: 1..4 segments", fn);
+  if (!seg_len) return fail(-1, "%s: invalid argument: null seg_len", fn);
+  long long tot = 0;
+  for (int s = 0; s < num_segments; ++s) {
+    if (seg_len[s] < 0) return fail(-1, "%s: invalid argument: negative segment length", fn);
+    begin[s] = tot;
+    tot += seg_len[s];
+  }
+  for (int s = num_segments; s <= kMaxSeg; ++s) begin[s] = tot;
+  if (n_total && tot != *n_total) return fail(-1, "%s: invalid argument: n_total != sum of segment lengths", fn);
+  return 0;
+}
+
 __device__ __forceinline__ int seg_of(const long long* begin, int nseg, long long g) {
   int s = 0;
 #pragma unroll

@@ -48,32 +48,144 @@ class KernelError(RuntimeError):
     pass
 
 
+class _QtOp(ctypes.Structure):       # mirrors `cutie_qt_op` (include/cutie_b200.h)
+    _fields_ = [('kind', ctypes.c_int32), ('phase', ctypes.c_int32), ('inp', ctypes.c_void_p * 8),
+                ('out', ctypes.c_void_p * 2), ('i', ctypes.c_int64 * 6), ('f', ctypes.c_float),
+                ('reserved', ctypes.c_int32)]
+
+
+# (restype, argtypes) of every entry point of include/cutie_b200.h, in the header's order.  With these ctypes converts
+# each Python argument to its C type and rejects one that does not convert (a float or str for an int64_t, say)
+# before the call, instead of passing a bare int as a 32-bit C int.
+_P, _I64, _INT, _SIZE, _F32 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_size_t, ctypes.c_float
+_BANK = (_INT,) + (_P,) * 5     # num_segments, seg_key, seg_shrinkage, seg_len, seg_key_bstride, seg_shr_bstride
+_CONV_TC = (_P,) * 6 + (_I64,) * 5 + (_INT,) * 4 + (_P, _P, _INT, _P, _P, _P)
+_SIGNATURES = {
+    'cutie_b200_abi_version': (_INT, ()),
+    'cutie_b200_last_error': (ctypes.c_char_p, ()),
+    'cutie_affinity_workspace_bytes': (_SIZE, (_I64, _I64, _I64, _INT)),
+    'cutie_affinity_topk': (_INT, _BANK + (_P, _P, _I64, _I64, _I64, _INT, _INT) + (_P,) * 4 + (_I64, _P, _SIZE, _P)),
+    'cutie_affinity_topk_img': (_INT, _BANK + (_P,) * 7 + (_I64, _I64, _I64, _INT, _INT) + (_P,) * 4
+                                + (_I64, _P, _SIZE, _P)),
+    'cutie_affinity_plan_levels': (_INT, (_I64, _INT)),
+    'cutie_debug_ws_count_offset': (_I64, (_I64, _I64, _I64, _INT)),
+    'cutie_set_tc_min_tokens': (None, (_I64,)),
+    'cutie_debug_phase_timing': (None, (_INT,)),
+    'cutie_debug_phase_times': (_INT, (_I64, _P, _INT)),
+    'cutie_debug_image_level_launches': (_I64, ()),
+    'cutie_debug_tc_energy': (_INT, _BANK + (_P, _P, _I64, _I64, _I64, _P, _P, _SIZE, _P)),
+    'cutie_topk_merge': (_INT, (_P, _P, _I64, _I64, _I64, _INT, _INT) + (_P,) * 4 + (_I64, _P)),
+    'cutie_readout_gather': (_INT, (_P, _P, _I64, _I64, _INT, _INT, _P, _P, _P, _I64, _I64, _P, _P)),
+    'cutie_usage_commit': (_INT, (_P, _I64, _P, _I64, _P, _I64, _I64, _I64, _I64, _P)),
+    'cutie_upsample2x_add': (_INT, (_P,) * 3 + (_I64,) * 5 + (_P,)),
+    'cutie_bias_act': (_INT, (_P,) * 3 + (_I64,) * 3 + (_INT, _INT, _P)),
+    'cutie_area_pool': (_INT, (_P, _P) + (_I64,) * 4 + (_P,)),
+    'cutie_eca_scale_add': (_INT, (_P,) * 5 + (_I64,) * 4 + (_INT, _P)),
+    'cutie_gated_update': (_INT, (_P,) * 3 + (_I64,) * 3 + (_P,)),
+    'cutie_bias_relu_maxpool': (_INT, (_P,) * 3 + (_I64,) * 4 + (_INT, _P)),
+    'cutie_segment_tail': (_INT, (_P,) * 4 + (_I64,) * 4 + (_P,)),
+    'cutie_conv_weight_image_bytes': (_I64, (_I64, _I64, _INT)),
+    'cutie_conv_weight_image': (_INT, (_P, _I64, _I64, _INT, _P, _P)),
+    'cutie_conv_tc': (_INT, _CONV_TC),
+    'cutie_conv_weight_image_f16_bytes': (_I64, (_I64, _I64, _INT)),
+    'cutie_conv_weight_image_f16': (_INT, (_P, _I64, _I64, _INT, _P, _P)),
+    'cutie_conv_tc_f16': (_INT, _CONV_TC),
+    'cutie_conv_plan': (_INT, (_I64,) * 5 + (_INT,) * 3 + (_P,)),
+    'cutie_debug_conv_tile_shape': (_INT, (_I64, _I64, _P)),
+    'cutie_conv3x3_c1': (_INT, (_P,) * 4 + (_I64,) * 4 + (_INT, _P)),
+    'cutie_prob_to_mask': (_INT, (_P,) + (_I64,) * 5 + (_P,) * 3),
+    'cutie_bank_append': (_INT, (_P, _I64, _P) + (_I64,) * 4 + (_P,)),
+    'cutie_bank_key_image': (_INT, (_P, _I64, _P) + (_I64,) * 4 + (_P, _I64, _I64, _P, _P)),
+    'cutie_bank_export': (_INT, (_P, _I64, _P) + (_I64,) * 4 + (_P,)),
+    'cutie_bank_gather': (_INT, (_INT,) + (_P,) * 5 + (_I64,) * 4 + (_P,)),
+    'cutie_consolidate': (_INT, _BANK + (_P, _P, _I64, _P, _I64, _P) + (_I64,) * 5 + (_P, _P, _P, _I64, _P, _I64, _P)),
+    'cutie_consolidate_partial': (_INT, _BANK + (_P, _P, _I64, _P, _I64, _P) + (_I64,) * 5
+                                  + (_P, _P, _P, _I64, _P, _P, _P, _I64, _P)),
+    'cutie_obj_summary_accumulate': (_INT, (_P, _P, _I64, _P)),
+    'cutie_qt_linear': (_INT, (_P, _I64, _I64, _P, _I64, _I64) + (_P,) * 4 + (_INT, _INT, _P, _I64, _P, _P, _P)),
+    'cutie_qt_head_fold': (_INT, (_P, _I64, _I64, _INT, _P, _I64, _INT, _F32) + (_P,) * 4),
+    'cutie_qt_self_attention': (_INT, (_P, _P, _I64, _I64, _INT, _INT, _P, _P)),
+    'cutie_qt_chain': (_INT, (ctypes.POINTER(_QtOp), _INT, _P, _P, _INT, _P, _P)),
+    'cutie_qt_aux_mask': (_INT, (_P,) * 3 + (_I64,) * 4 + (_P,) * 4),
+    'cutie_qt_mask_logits': (_INT, (_P,) * 3 + (_I64,) * 4 + (_P, _P)),
+    'cutie_qt_aux_fg': (_INT, (_P, _P) + (_I64,) * 4 + (_P,) * 3),
+    'cutie_qt_pixel_to_query_splits': (_INT, (_I64, _I64, _INT)),
+    'cutie_qt_pixel_to_query_workspace_floats': (_I64, (_I64, _I64)),
+    'cutie_qt_pixel_to_query': (_INT, (_P,) * 6 + (_I64, _P, _I64, _I64, _I64, _INT, _INT, _INT, _P, _P, _P)),
+    'cutie_qt_query_to_pixel': (_INT, (_P,) * 6 + (_I64, _I64, _I64, _INT, _INT, _P, _P)),
+}
+
+
+def _declare(f, name: str):
+    f.restype, f.argtypes = _SIGNATURES[name]
+    return f
+
+
+def bind(cdll: ctypes.CDLL) -> ctypes.CDLL:
+    """Declare the C signature of every entry point `cdll` exports (a library that exports only some, such as a host
+    build of one source file, gets those)."""
+    for name in _SIGNATURES:
+        f = getattr(cdll, name, None)
+        if f is not None:
+            _declare(f, name)
+    return cdll
+
+
 def lib() -> ctypes.CDLL:
     global _lib
     if _lib is None:
         if not os.path.exists(_LIB_PATH):
             raise KernelError(f'{_LIB_PATH} not found: build it with `python __graft_entry__.py build` '
                               '(there is no CPU or PyTorch fallback for the Cutie hot path)')
-        _lib = ctypes.CDLL(_LIB_PATH)
-        _lib.cutie_b200_last_error.restype = ctypes.c_char_p
-        _lib.cutie_affinity_workspace_bytes.restype = ctypes.c_size_t
-        _lib.cutie_affinity_workspace_bytes.argtypes = [ctypes.c_int64] * 3 + [ctypes.c_int]
+        _lib = bind(ctypes.CDLL(_LIB_PATH))
     return _lib
+
+
+def _entry(name: str):
+    """Entry point `name` of lib() with its C signature declared, whichever library lib() returns (tests substitute a
+    host build of one source file for it)."""
+    f = getattr(lib(), name)
+    return f if f.argtypes is not None else _declare(f, name)
 
 
 def _check(status: int, what: str):
     if status != 0:
-        msg = lib().cutie_b200_last_error()
+        msg = _entry('cutie_b200_last_error')()
         raise KernelError(f'{what} failed (status {status}): {msg.decode() if msg else "?"}')
 
 
-def _stream() -> ctypes.c_void_p:
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+def _stream() -> int:
+    return torch.cuda.current_stream().cuda_stream
 
 
-def _ptr(t: Optional[torch.Tensor], dtype=torch.float32) -> ctypes.c_void_p:
+def _launch(name: str, fn: str, launches: int, *args):
+    """Enqueue the C entry point `fn` with `args` and the current stream, counted and profiled as `name` (_call);
+    a non-zero status raises KernelError."""
+    with _call(name, launches):
+        st = _entry(fn)(*args, _stream())
+    _check(st, fn)
+
+
+def _array(ctype, values) -> ctypes.Array:
+    values = list(values)
+    return (ctype * len(values))(*values)
+
+
+def _rows_arrays(tensors: Sequence[torch.Tensor]):
+    """(pointers, batch strides) of a list of token-major row tensors: the per-segment arrays of the C-ABI."""
+    return _array(ctypes.c_void_p, (t.data_ptr() for t in tensors)), _array(ctypes.c_int64, (t.stride(0) for t in tensors))
+
+
+def _bank_arrays(segments: Sequence['BankSegment']):
+    """The bank arguments (num_segments, seg_key, seg_shrinkage, seg_len, seg_key_bstride, seg_shr_bstride)."""
+    keys, key_bs = _rows_arrays([s.key for s in segments])
+    shrs, shr_bs = _rows_arrays([s.shrinkage for s in segments])
+    return len(segments), keys, shrs, _array(ctypes.c_int64, (s.n for s in segments)), key_bs, shr_bs
+
+
+def _ptr(t: Optional[torch.Tensor], dtype=torch.float32) -> Optional[int]:
     if t is None:
-        return ctypes.c_void_p(0)
+        return None
     if not t.is_cuda:
         raise KernelError('cutie_b200 kernels need CUDA tensors (no CPU path exists)')
     if t.device.index != torch.cuda.current_device():
@@ -83,11 +195,7 @@ def _ptr(t: Optional[torch.Tensor], dtype=torch.float32) -> ctypes.c_void_p:
                           '(wrap the call in torch.cuda.device(tensor.device))')
     if t.dtype != dtype:
         raise KernelError(f'expected {dtype}, got {t.dtype}')
-    return ctypes.c_void_p(t.data_ptr())
-
-
-def _i64(v) -> ctypes.c_int64:
-    return ctypes.c_int64(int(v))
+    return t.data_ptr()
 
 
 class BankSegment(NamedTuple):
@@ -157,18 +265,14 @@ def affinity_topk(segments: Sequence[BankSegment], qk: torch.Tensor, qe: torch.T
     idx = torch.empty(B, Q, kpad, dtype=torch.int32, device=dev)
     w = torch.empty(B, Q, kpad, dtype=torch.float32, device=dev)
     sim = torch.empty(B, Q, kpad, dtype=torch.float32, device=dev) if want_sim else None
-    L = lib()
-    ws_bytes = L.cutie_affinity_workspace_bytes(B, Q, n_total, top_k)
+    ws_bytes = _entry('cutie_affinity_workspace_bytes')(B, Q, n_total, top_k)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    ns = len(segments)
-    assert 1 <= ns <= 4
+    assert 1 <= len(segments) <= 4
     for s in segments:
         _rows_view_ok(s.key), _rows_view_ok(s.shrinkage)
         assert s.key.shape[2] == CK
     assert qk.is_contiguous() and qe.is_contiguous()
-    PA, IA = ctypes.c_void_p * ns, ctypes.c_int64 * ns
-    _L = lib()
-    _lv = _L.cutie_affinity_plan_levels(_i64(n_total), ctypes.c_int(top_k))
+    levels = affinity_plan_levels(n_total, top_k)
     with_img = all(s.key_image is not None for s in segments)
     if with_img:
         for s in segments:
@@ -183,21 +287,15 @@ def affinity_topk(segments: Sequence[BankSegment], qk: torch.Tensor, qe: torch.T
             assert mu.shape == (B, CK) and mu.is_contiguous()
         if seed_idx is not None:
             assert seed_idx.shape == (B, Q, kpad) and seed_idx.is_contiguous()
-        img_args = (PA(*[s.key_image.data_ptr() for s in segments]), IA(*[s.key_image.stride(0) for s in segments]),
-                    IA(*[s.phys_begin for s in segments]), _ptr(mu), _ptr(seed_idx, torch.int32))
+        img_args = (*_rows_arrays([s.key_image for s in segments]), _array(ctypes.c_int64, (s.phys_begin for s in segments)),
+                    _ptr(mu), _ptr(seed_idx, torch.int32))
     else:
-        img_args = (None, None, None, None, None)
+        img_args = (None,) * 5
     # launches: exact scan = scan + merge; FP16 image plan = sample pass, threshold, filter pass, re-rank; TF32 levels
     # (no image) = one filter per level, a select between levels, re-rank
-    with _call('affinity_topk', (4 if with_img else 2 * _lv) if _lv else 2):
-        st = L.cutie_affinity_topk_img(
-            ctypes.c_int(ns), PA(*[s.key.data_ptr() for s in segments]),
-            PA(*[s.shrinkage.data_ptr() for s in segments]), IA(*[s.n for s in segments]),
-            IA(*[s.key.stride(0) for s in segments]), IA(*[s.shrinkage.stride(0) for s in segments]),
-            *img_args, _ptr(qk), _ptr(qe), _i64(B), _i64(CK), _i64(Q), ctypes.c_int(top_k), ctypes.c_int(kpad),
-            _ptr(idx, torch.int32), _ptr(w), _ptr(sim), _ptr(usage_acc, torch.int64), _i64(n_total),
-            _ptr(ws, torch.uint8), ctypes.c_size_t(ws_bytes), _stream())
-    _check(st, 'cutie_affinity_topk')
+    _launch('affinity_topk', 'cutie_affinity_topk_img', (4 if with_img else 2 * levels) if levels else 2,
+            *_bank_arrays(segments), *img_args, _ptr(qk), _ptr(qe), B, CK, Q, top_k, kpad, _ptr(idx, torch.int32),
+            _ptr(w), _ptr(sim), _ptr(usage_acc, torch.int64), n_total, _ptr(ws, torch.uint8), ws_bytes)
     if KEEP_LAST_WORKSPACE:
         global _LAST_WS
         _LAST_WS = (ws, B, Q, n_total, top_k)
@@ -214,9 +312,7 @@ def last_candidate_counts() -> Optional[torch.Tensor]:
     if _LAST_WS is None:
         return None
     ws, B, Q, n_total, top_k = _LAST_WS
-    f = lib().cutie_debug_ws_count_offset
-    f.restype = ctypes.c_int64
-    off = int(f(_i64(B), _i64(Q), _i64(n_total), ctypes.c_int(top_k)))
+    off = _entry('cutie_debug_ws_count_offset')(B, Q, n_total, top_k)
     if off < 0:
         return None
     return ws[off:off + 4 * B * Q].view(torch.int32).view(B, Q).clone()
@@ -224,31 +320,29 @@ def last_candidate_counts() -> Optional[torch.Tensor]:
 
 def set_tc_min_tokens(n: int):
     """Banks with fewer tokens than n use the exact fp32 scan only; larger ones add the wgmma filter levels."""
-    lib().cutie_set_tc_min_tokens(_i64(n))
+    _entry('cutie_set_tc_min_tokens')(n)
 
 
 def phase_timing(enable: bool):
     """Record per-launch device times inside the filtered affinity plan (diagnostics)."""
-    lib().cutie_debug_phase_timing(ctypes.c_int(1 if enable else 0))
+    _entry('cutie_debug_phase_timing')(1 if enable else 0)
 
 
 def phase_times(calls_ago: int = 0):
     """[ms per phase] of the affinity call `calls_ago` calls back: filter, select, filter, select, ..., re-rank."""
     buf = (ctypes.c_float * 16)()
-    n = lib().cutie_debug_phase_times(_i64(calls_ago), buf, ctypes.c_int(16))
+    n = _entry('cutie_debug_phase_times')(calls_ago, buf, 16)
     return [float(buf[i]) for i in range(n)]
 
 
 def image_level_launches() -> int:
     """How many filter levels this process has served from a key image (bulk-copy producer) so far."""
-    f = lib().cutie_debug_image_level_launches
-    f.restype = ctypes.c_int64
-    return int(f())
+    return _entry('cutie_debug_image_level_launches')()
 
 
 def affinity_plan_levels(n_total: int, top_k: int) -> int:
     """0 = exact fp32 scan only; n >= 1 = n nested wgmma filter levels + exact re-rank of the survivors."""
-    return int(lib().cutie_affinity_plan_levels(_i64(n_total), ctypes.c_int(top_k)))
+    return _entry('cutie_affinity_plan_levels')(n_total, top_k)
 
 
 def debug_tc_energy(segments: Sequence[BankSegment], qk: torch.Tensor, qe: torch.Tensor) -> torch.Tensor:
@@ -256,18 +350,10 @@ def debug_tc_energy(segments: Sequence[BankSegment], qk: torch.Tensor, qe: torch
     B, CK, Q = qk.shape
     n_total = sum(s.n for s in segments)
     out = torch.zeros(B, Q, n_total, dtype=torch.float32, device=qk.device)
-    ns = len(segments)
-    PA, IA = ctypes.c_void_p * ns, ctypes.c_int64 * ns
     ws_bytes = B * Q * (16384 * 8 + 16 + 32 * 8) + (1 << 20)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=qk.device)
-    with _call('debug_tc_energy', 2):
-        st = lib().cutie_debug_tc_energy(
-            ctypes.c_int(ns), PA(*[s.key.data_ptr() for s in segments]),
-            PA(*[s.shrinkage.data_ptr() for s in segments]), IA(*[s.n for s in segments]),
-            IA(*[s.key.stride(0) for s in segments]), IA(*[s.shrinkage.stride(0) for s in segments]),
-            _ptr(qk), _ptr(qe), _i64(B), _i64(Q), _i64(n_total), _ptr(out), _ptr(ws, torch.uint8),
-            ctypes.c_size_t(ws_bytes), _stream())
-    _check(st, 'cutie_debug_tc_energy')
+    _launch('debug_tc_energy', 'cutie_debug_tc_energy', 2, *_bank_arrays(segments), _ptr(qk), _ptr(qe), B, Q, n_total,
+            _ptr(out), _ptr(ws, torch.uint8), ws_bytes)
     return out
 
 
@@ -281,11 +367,8 @@ def topk_merge(part_val: torch.Tensor, part_idx: torch.Tensor, top_k: int, n_tot
     idx = torch.empty(B, Q, kpad, dtype=torch.int32, device=dev)
     w = torch.empty(B, Q, kpad, dtype=torch.float32, device=dev)
     sim = torch.empty(B, Q, kpad, dtype=torch.float32, device=dev) if want_sim else None
-    with _call('topk_merge', 1):
-        st = lib().cutie_topk_merge(_ptr(part_val), _ptr(part_idx, torch.int32), _i64(B), _i64(parts), _i64(Q),
-                                    ctypes.c_int(top_k), ctypes.c_int(kpad), _ptr(idx, torch.int32), _ptr(w),
-                                    _ptr(sim), _ptr(usage_acc, torch.int64), _i64(n_total), _stream())
-    _check(st, 'cutie_topk_merge')
+    _launch('topk_merge', 'cutie_topk_merge', 1, _ptr(part_val), _ptr(part_idx, torch.int32), B, parts, Q, top_k, kpad,
+            _ptr(idx, torch.int32), _ptr(w), _ptr(sim), _ptr(usage_acc, torch.int64), n_total)
     return idx, w, sim
 
 
@@ -299,21 +382,14 @@ def readout_gather(idx: torch.Tensor, w: torch.Tensor, segments: Sequence[BankSe
     CV = segments[0].values[0].shape[2]
     if out is None:
         out = torch.empty(B, K, CV, Q, dtype=torch.float32, device=idx.device)
-    ns = len(segments)
-    ptrs, strides = [], []
+    values = []
     for s in segments:
         assert len(s.values) == K
         for v in s.values:
             _rows_view_ok(v)
-            ptrs.append(v.data_ptr())
-            strides.append(v.stride(0))
-    PA, IA, IS = ctypes.c_void_p * (ns * K), ctypes.c_int64 * (ns * K), ctypes.c_int64 * ns
-    _L = lib()
-    with _call('readout_gather', -(-K // 16)):
-        st = _L.cutie_readout_gather(_ptr(idx, torch.int32), _ptr(w), _i64(B), _i64(Q), ctypes.c_int(kpad),
-                                        ctypes.c_int(ns), IS(*[s.n for s in segments]), PA(*ptrs), IA(*strides),
-                                        _i64(K), _i64(CV), _ptr(out), _stream())
-    _check(st, 'cutie_readout_gather')
+        values += s.values
+    _launch('readout_gather', 'cutie_readout_gather', -(-K // 16), _ptr(idx, torch.int32), _ptr(w), B, Q, kpad,
+            len(segments), _array(ctypes.c_int64, (s.n for s in segments)), *_rows_arrays(values), K, CV, _ptr(out))
     return out
 
 
@@ -322,11 +398,8 @@ def usage_commit(use_cnt: torch.Tensor, life_cnt: torch.Tensor, usage_acc: torch
     B, n = use_cnt.shape
     if n == 0:
         return
-    with _call('usage_commit', 1):
-        st = lib().cutie_usage_commit(_ptr(use_cnt), _i64(use_cnt.stride(0)), _ptr(life_cnt), _i64(life_cnt.stride(0)),
-                                      _ptr(usage_acc, torch.int64), _i64(usage_acc.stride(0)), _i64(acc_offset),
-                                      _i64(B), _i64(n), _stream())
-    _check(st, 'cutie_usage_commit')
+    _launch('usage_commit', 'cutie_usage_commit', 1, _ptr(use_cnt), use_cnt.stride(0), _ptr(life_cnt), life_cnt.stride(0),
+            _ptr(usage_acc, torch.int64), usage_acc.stride(0), acc_offset, B, n)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -338,10 +411,7 @@ def bank_append(src: torch.Tensor, dst_rows: torch.Tensor):
     assert dst_rows.shape == (B, n, C)
     _rows_view_ok(dst_rows)
     assert src.stride(2) == 1 and src.stride(1) == n
-    with _call('bank_append', 1):
-        st = lib().cutie_bank_append(_ptr(src), _i64(src.stride(0)), _ptr(dst_rows), _i64(dst_rows.stride(0)),
-                                     _i64(B), _i64(C), _i64(n), _stream())
-    _check(st, 'cutie_bank_append')
+    _launch('bank_append', 'cutie_bank_append', 1, _ptr(src), src.stride(0), _ptr(dst_rows), dst_rows.stride(0), B, C, n)
 
 
 def upsample2x_add(g: torch.Tensor, skip: torch.Tensor) -> torch.Tensor:
@@ -351,10 +421,7 @@ def upsample2x_add(g: torch.Tensor, skip: torch.Tensor) -> torch.Tensor:
     assert skip.shape == (B, C, 2 * h, 2 * w)
     g, skip = g.contiguous(), skip.contiguous()
     out = torch.empty(B, K, C, 2 * h, 2 * w, dtype=torch.float32, device=g.device)
-    with _call('upsample2x_add', 1):
-        st = lib().cutie_upsample2x_add(_ptr(g), _ptr(skip), _ptr(out), _i64(B), _i64(K), _i64(C), _i64(h), _i64(w),
-                                        _stream())
-    _check(st, 'cutie_upsample2x_add')
+    _launch('upsample2x_add', 'cutie_upsample2x_add', 1, _ptr(g), _ptr(skip), _ptr(out), B, K, C, h, w)
     return out
 
 
@@ -375,10 +442,7 @@ def bias_act_(y: torch.Tensor, bias: torch.Tensor, z: Optional[torch.Tensor] = N
             z = torch.empty_like(y).copy_(z)
     bias = bias.detach()
     assert bias.shape == (C,) and bias.is_contiguous()
-    with _call('bias_act', 1):
-        st = lib().cutie_bias_act(_ptr(y), _ptr(bias), _ptr(z), _i64(N), _i64(C), _i64(H * W), int(cl), int(bool(relu)),
-                                  _stream())
-    _check(st, 'cutie_bias_act')
+    _launch('bias_act', 'cutie_bias_act', 1, _ptr(y), _ptr(bias), _ptr(z), N, C, H * W, cl, relu)
     return y
 
 
@@ -398,10 +462,7 @@ def bias_relu_maxpool(y: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
                       memory_format=torch.channels_last if cl else torch.contiguous_format)
     bias = bias.detach()
     assert bias.shape == (C,) and bias.is_contiguous()
-    with _call('bias_relu_maxpool', 1):
-        st = lib().cutie_bias_relu_maxpool(_ptr(y), _ptr(bias), _ptr(out), _i64(N), _i64(C), _i64(H), _i64(W), int(cl),
-                                           _stream())
-    _check(st, 'cutie_bias_relu_maxpool')
+    _launch('bias_relu_maxpool', 'cutie_bias_relu_maxpool', 1, _ptr(y), _ptr(bias), _ptr(out), N, C, H, W, cl)
     return out
 
 
@@ -417,10 +478,7 @@ def segment_tail(x: torch.Tensor):
     agg = torch.empty(B, K + 1, h, w, dtype=torch.float32, device=x.device)
     logits = torch.empty(B, K + 1, 4 * h, 4 * w, dtype=torch.float32, device=x.device)
     prob = torch.empty_like(logits)
-    with _call('segment_tail', 2):
-        st = lib().cutie_segment_tail(_ptr(x), _ptr(agg), _ptr(logits), _ptr(prob), _i64(B), _i64(K), _i64(h), _i64(w),
-                                      _stream())
-    _check(st, 'cutie_segment_tail')
+    _launch('segment_tail', 'cutie_segment_tail', 2, _ptr(x), _ptr(agg), _ptr(logits), _ptr(prob), B, K, h, w)
     return logits, prob
 
 
@@ -431,10 +489,7 @@ def conv3x3_c1(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, relu_i
     x = x.contiguous()
     w = weight.detach().contiguous()
     out = torch.empty(N, 1, H, W, dtype=torch.float32, device=x.device)
-    with _call('conv3x3_c1', 1):
-        st = lib().cutie_conv3x3_c1(_ptr(x), _ptr(w), _ptr(bias.detach()), _ptr(out), _i64(N), _i64(C), _i64(H), _i64(W),
-                                    int(bool(relu_input)), _stream())
-    _check(st, 'cutie_conv3x3_c1')
+    _launch('conv3x3_c1', 'cutie_conv3x3_c1', 1, _ptr(x), _ptr(w), _ptr(bias.detach()), _ptr(out), N, C, H, W, relu_input)
     return out
 
 
@@ -454,9 +509,7 @@ def conv_tc_eligible(weight: torch.Tensor, stride=(1, 1), padding=(1, 1), dilati
 
 def conv_weight_image_bytes(cout: int, cin: int, ksize: int, f16: bool = False) -> int:
     """Bytes of a layer's operand image for cutie_conv_tc (f16=False) or cutie_conv_tc_f16 (f16=True); -1: no such image."""
-    f = lib().cutie_conv_weight_image_f16_bytes if f16 else lib().cutie_conv_weight_image_bytes
-    f.restype = ctypes.c_int64
-    return int(f(_i64(cout), _i64(cin), int(ksize)))
+    return _entry('cutie_conv_weight_image_f16_bytes' if f16 else 'cutie_conv_weight_image_bytes')(cout, cin, ksize)
 
 
 def _conv_weight_image(weight: torch.Tensor, f16: bool) -> torch.Tensor:
@@ -464,10 +517,8 @@ def _conv_weight_image(weight: torch.Tensor, f16: bool) -> torch.Tensor:
     assert weight.dtype == torch.float32 and weight.shape[2] == weight.shape[3] and k in (1, 3) and Cin % 32 == 0
     img = torch.empty(conv_weight_image_bytes(Cout, Cin, k, f16) // 4, dtype=torch.float32, device=weight.device)
     w = weight.detach().contiguous()
-    name = 'conv_weight_image_f16' if f16 else 'conv_weight_image'
-    with _call(name, 1):
-        st = getattr(lib(), 'cutie_' + name)(_ptr(w), _i64(Cout), _i64(Cin), int(k), _ptr(img), _stream())
-    _check(st, 'cutie_' + name)
+    name, fn = ('conv_weight_image_f16', 'cutie_conv_weight_image_f16') if f16 else ('conv_weight_image', 'cutie_conv_weight_image')
+    _launch(name, fn, 1, _ptr(w), Cout, Cin, k, _ptr(img))
     return img
 
 
@@ -528,24 +579,18 @@ def conv_tc(x: torch.Tensor, weight_image: torch.Tensor, bias: Optional[torch.Te
         if zs is None:
             residual = residual.contiguous()
             zs = _ncp_strides(residual)
-    arr = lambda t: (ctypes.c_int64 * 3)(*t)
     plan = (ctypes.c_int64 * 6)()
     q = int(units_per_cta) if units_per_cta else 0
-    _check(lib().cutie_conv_plan(_i64(N), _i64(Cin), _i64(cout), _i64(H), _i64(W), int(ksize), int(stride), q, plan),
-           'cutie_conv_plan')
-    ntile, ws_floats = int(plan[0]), int(plan[5])
+    _check(_entry('cutie_conv_plan')(N, Cin, cout, H, W, ksize, stride, q, plan), 'cutie_conv_plan')
+    ntile, ws_floats = plan[0], plan[5]
     ws = cnt = None
     if ws_floats:
         ws = torch.empty(ws_floats, dtype=torch.float32, device=x.device)
         cnt = counters if counters is not None and counters.numel() >= ntile else torch.zeros(ntile, dtype=torch.int32, device=x.device)
-    name = 'conv_tc_f16' if f16 else 'conv_tc'
-    with _call(name, 1):
-        st = getattr(lib(), 'cutie_' + name)(
-            _ptr(x), arr(_ncp_strides(x)), _ptr(weight_image), _ptr(bias),
-            _ptr(residual), arr(zs) if zs is not None else None, _i64(N), _i64(Cin), _i64(cout), _i64(H), _i64(W),
-            int(ksize), int(stride), int(bool(relu_in)), int(bool(relu_out)), _ptr(out), arr(_ncp_strides(out)), q,
-            _ptr(ws), _ptr(cnt, torch.int32), _stream())
-    _check(st, 'cutie_' + name)
+    name, fn = ('conv_tc_f16', 'cutie_conv_tc_f16') if f16 else ('conv_tc', 'cutie_conv_tc')
+    _launch(name, fn, 1, _ptr(x), _array(ctypes.c_int64, _ncp_strides(x)), _ptr(weight_image), _ptr(bias), _ptr(residual),
+            _array(ctypes.c_int64, zs) if zs is not None else None, N, Cin, cout, H, W, ksize, stride, relu_in, relu_out,
+            _ptr(out), _array(ctypes.c_int64, _ncp_strides(out)), q, _ptr(ws), _ptr(cnt, torch.int32))
     return out
 
 
@@ -561,9 +606,7 @@ def area_pool(x: torch.Tensor, f: int) -> torch.Tensor:
     x = x.contiguous()
     out = torch.empty(*x.shape[:-2], H // f, W // f, dtype=torch.float32, device=x.device)
     planes = x.numel() // (H * W)
-    with _call('area_pool', 1):
-        st = lib().cutie_area_pool(_ptr(x), _ptr(out), _i64(planes), _i64(H), _i64(W), _i64(f), _stream())
-    _check(st, 'cutie_area_pool')
+    _launch('area_pool', 'cutie_area_pool', 1, _ptr(x), _ptr(out), planes, H, W, f)
     return out
 
 
@@ -583,10 +626,8 @@ def eca_scale_add_(y: torch.Tensor, x: torch.Tensor, conv1d_weight: torch.Tensor
     w = conv1d_weight.detach().reshape(-1)
     mean = y.mean(dim=(2, 3)).contiguous()
     gate = torch.empty_like(mean)
-    with _call('eca_scale_add', 2):
-        st = lib().cutie_eca_scale_add(_ptr(y), _ptr(x), _ptr(mean), _ptr(w), _ptr(gate), _i64(N), _i64(C), _i64(H * W),
-                                       _i64(w.numel()), int(cl), _stream())
-    _check(st, 'cutie_eca_scale_add')
+    _launch('eca_scale_add', 'cutie_eca_scale_add', 2, _ptr(y), _ptr(x), _ptr(mean), _ptr(w), _ptr(gate), N, C, H * W,
+            w.numel(), cl)
     return y
 
 
@@ -596,9 +637,7 @@ def gated_update(h: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
     assert v.shape == (B, K, 3 * d, H, W) and h.dtype == torch.float32 and v.dtype == torch.float32
     h, v = h.contiguous(), v.contiguous()
     out = torch.empty_like(h)
-    with _call('gated_update', 1):
-        st = lib().cutie_gated_update(_ptr(v), _ptr(h), _ptr(out), _i64(B * K), _i64(d), _i64(H * W), _stream())
-    _check(st, 'cutie_gated_update')
+    _launch('gated_update', 'cutie_gated_update', 1, _ptr(v), _ptr(h), _ptr(out), B * K, d, H * W)
     return out
 
 
@@ -607,10 +646,8 @@ def prob_to_mask(prob: torch.Tensor, lut: torch.Tensor) -> torch.Tensor:
     C, H, W = prob.shape
     assert prob.stride(2) == 1 and lut.dtype == torch.int64 and lut.numel() >= C and lut.is_contiguous()
     out = torch.empty(H, W, dtype=torch.int64, device=prob.device)
-    with _call('prob_to_mask', 1):
-        st = lib().cutie_prob_to_mask(_ptr(prob), _i64(prob.stride(0)), _i64(prob.stride(1)), _i64(C), _i64(H), _i64(W),
-                                      _ptr(lut, torch.int64), _ptr(out, torch.int64), _stream())
-    _check(st, 'cutie_prob_to_mask')
+    _launch('prob_to_mask', 'cutie_prob_to_mask', 1, _ptr(prob), prob.stride(0), prob.stride(1), C, H, W,
+            _ptr(lut, torch.int64), _ptr(out, torch.int64))
     return out
 
 
@@ -634,11 +671,8 @@ def bank_key_image(key_arena: torch.Tensor, shr_arena: torch.Tensor, phys_begin:
     assert image.stride(2) == 1 and image.stride(1) == KEY_IMAGE_FLOATS
     assert 0 <= phys_begin and phys_begin + n <= cap
     assert mu is None or (mu.shape == (B, CK) and mu.is_contiguous())
-    with _call('bank_key_image', 1):
-        st = lib().cutie_bank_key_image(_ptr(key_arena), _i64(key_arena.stride(0)), _ptr(shr_arena),
-                                        _i64(shr_arena.stride(0)), _i64(B), _i64(phys_begin), _i64(n), _ptr(image),
-                                        _i64(image.stride(0)), _i64(image.shape[1]), _ptr(mu), _stream())
-    _check(st, 'cutie_bank_key_image')
+    _launch('bank_key_image', 'cutie_bank_key_image', 1, _ptr(key_arena), key_arena.stride(0), _ptr(shr_arena),
+            shr_arena.stride(0), B, phys_begin, n, _ptr(image), image.stride(0), image.shape[1], _ptr(mu))
 
 
 def bank_export(rows: torch.Tensor, dst: torch.Tensor):
@@ -646,10 +680,7 @@ def bank_export(rows: torch.Tensor, dst: torch.Tensor):
     B, n, C = rows.shape
     assert dst.shape == (B, C, n) and dst.is_contiguous()
     _rows_view_ok(rows)
-    with _call('bank_export', 1):
-        st = lib().cutie_bank_export(_ptr(rows), _i64(rows.stride(0)), _ptr(dst), _i64(dst.stride(0)),
-                                     _i64(B), _i64(C), _i64(n), _stream())
-    _check(st, 'cutie_bank_export')
+    _launch('bank_export', 'cutie_bank_export', 1, _ptr(rows), rows.stride(0), _ptr(dst), dst.stride(0), B, C, n)
 
 
 def bank_gather(segments_rows: Sequence[torch.Tensor], index: torch.Tensor, dst_rows: torch.Tensor):
@@ -658,18 +689,14 @@ def bank_gather(segments_rows: Sequence[torch.Tensor], index: torch.Tensor, dst_
     B, m = index.shape
     C = dst_rows.shape[2]
     assert dst_rows.shape[:2] == (B, m)
-    ns = len(segments_rows)
-    assert 1 <= ns <= 4
+    assert 1 <= len(segments_rows) <= 4
     for r in segments_rows:
         _rows_view_ok(r)
     _rows_view_ok(dst_rows)
-    PA, IA = ctypes.c_void_p * ns, ctypes.c_int64 * ns
-    with _call('bank_gather', 1):
-        st = lib().cutie_bank_gather(ctypes.c_int(ns), PA(*[r.data_ptr() for r in segments_rows]),
-                                     IA(*[r.shape[1] for r in segments_rows]), IA(*[r.stride(0) for r in segments_rows]),
-                                     _ptr(index, torch.int64), _ptr(dst_rows), _i64(dst_rows.stride(0)),
-                                     _i64(B), _i64(m), _i64(C), _stream())
-    _check(st, 'cutie_bank_gather')
+    rows, rows_bs = _rows_arrays(segments_rows)
+    _launch('bank_gather', 'cutie_bank_gather', 1, len(segments_rows), rows,
+            _array(ctypes.c_int64, (r.shape[1] for r in segments_rows)), rows_bs, _ptr(index, torch.int64), _ptr(dst_rows),
+            dst_rows.stride(0), B, m, C)
 
 
 def consolidate(segments: Sequence[BankSegment], proto_key: torch.Tensor, proto_sel: torch.Tensor,
@@ -685,41 +712,26 @@ def consolidate(segments: Sequence[BankSegment], proto_key: torch.Tensor, proto_
     once per group of 16 objects, and object k's rows are the same bits as in a call with object k alone.
     """
     B, P, CK = proto_key.shape
-    ns = len(segments)
     K = len(out_values)
     n_total = sum(s.n for s in segments)
     ws = torch.empty(B * P * n_total, dtype=torch.float32, device=proto_key.device)
-    PA, IA = ctypes.c_void_p * ns, ctypes.c_int64 * ns
-    VA, VI = ctypes.c_void_p * (ns * K), ctypes.c_int64 * (ns * K)
-    OA, OI = ctypes.c_void_p * K, ctypes.c_int64 * K
-    vp, vs = [], []
-    for s in segments:
-        for v in s.values:
-            vp.append(v.data_ptr()), vs.append(v.stride(0))
     for t in (proto_key, proto_sel):
         _rows_view_ok(t)
     if stats is not None:
         for t in stats:
             assert t.shape == (B, P) and t.is_contiguous() and t.dtype == torch.float32
-    with _call('consolidate', max(1, -(-K // 16))):
-        st = lib().cutie_consolidate_partial(
-            ctypes.c_int(ns), PA(*[s.key.data_ptr() for s in segments]), PA(*[s.shrinkage.data_ptr() for s in segments]),
-            IA(*[s.n for s in segments]), IA(*[s.key.stride(0) for s in segments]),
-            IA(*[s.shrinkage.stride(0) for s in segments]), VA(*vp), VI(*vs), _i64(K),
-            _ptr(proto_key), _i64(proto_key.stride(0)), _ptr(proto_sel), _i64(proto_sel.stride(0)),
-            _i64(B), _i64(P), _i64(CK), _i64(out_values[0].shape[2] if K else 0),
-            OA(*[v.data_ptr() for v in out_values]), OI(*[v.stride(0) for v in out_values]),
-            _ptr(out_shrinkage), _i64(out_shrinkage.stride(0)), _ptr(stats[0] if stats else None),
-            _ptr(stats[1] if stats else None), _ptr(ws), _i64(n_total), _stream())
-    _check(st, 'cutie_consolidate_partial')
+    _launch('consolidate', 'cutie_consolidate_partial', max(1, -(-K // 16)),
+            *_bank_arrays(segments), *_rows_arrays([v for s in segments for v in s.values]), K,
+            _ptr(proto_key), proto_key.stride(0), _ptr(proto_sel), proto_sel.stride(0),
+            B, P, CK, out_values[0].shape[2] if K else 0, *_rows_arrays(out_values),
+            _ptr(out_shrinkage), out_shrinkage.stride(0), _ptr(stats[0] if stats else None),
+            _ptr(stats[1] if stats else None), _ptr(ws), n_total)
 
 
 def obj_summary_accumulate(acc: torch.Tensor, new: torch.Tensor):
     """acc += new  (streaming object-memory sum, memory_manager.py:252-271).  Both [B, Q, E+1] dense."""
     assert acc.is_contiguous() and new.is_contiguous() and acc.shape == new.shape
-    with _call('obj_summary_accumulate', 1):
-        st = lib().cutie_obj_summary_accumulate(_ptr(acc), _ptr(new), _i64(acc.numel()), _stream())
-    _check(st, 'cutie_obj_summary_accumulate')
+    _launch('obj_summary_accumulate', 'cutie_obj_summary_accumulate', 1, _ptr(acc), _ptr(new), acc.numel())
 
 
 # ---------------------------------------------------------------------------------------------
@@ -745,12 +757,9 @@ def qt_linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor
         out = torch.empty(M, N, dtype=torch.float32, device=x.device)
     if ln is not None:
         assert Kd == 256, 'fused LayerNorm supports embed_dim 256'
-    with _call('qt_linear', 1):
-        st = lib().cutie_qt_linear(
-            _ptr(x), _i64(M), _i64(Kd), _ptr(weight), _i64(weight.stride(0)), _i64(N), _ptr(bias),
-            _ptr(ln[0] if ln else None), _ptr(ln[1] if ln else None), _ptr(pe), ctypes.c_int(int(summary_norm)),
-            ctypes.c_int(int(relu)), _ptr(residual), _i64(residual_mod), _ptr(xhat_out), _ptr(out), _stream())
-    _check(st, 'cutie_qt_linear')
+    _launch('qt_linear', 'cutie_qt_linear', 1, _ptr(x), M, Kd, _ptr(weight), weight.stride(0), N, _ptr(bias),
+            _ptr(ln[0] if ln else None), _ptr(ln[1] if ln else None), _ptr(pe), summary_norm, relu, _ptr(residual),
+            residual_mod, _ptr(xhat_out), _ptr(out))
     return out
 
 
@@ -765,11 +774,8 @@ def qt_head_fold(a: torch.Tensor, weight: torch.Tensor, *, transpose_w: bool, sc
     assert weight.shape == (E, E) and weight.stride(1) == 1
     out = torch.empty(M, num_heads, E, dtype=torch.float32, device=a.device)
     dots = torch.empty(M, num_heads, dtype=torch.float32, device=a.device) if bias_vec is not None else None
-    with _call('qt_head_fold', 1):
-        st = lib().cutie_qt_head_fold(_ptr(a), _i64(M), _i64(E), ctypes.c_int(num_heads), _ptr(weight),
-                                      _i64(weight.stride(0)), ctypes.c_int(int(transpose_w)), ctypes.c_float(scale),
-                                      _ptr(bias_vec), _ptr(out), _ptr(dots), _stream())
-    _check(st, 'cutie_qt_head_fold')
+    _launch('qt_head_fold', 'cutie_qt_head_fold', 1, _ptr(a), M, E, num_heads, _ptr(weight), weight.stride(0), transpose_w,
+            scale, _ptr(bias_vec), _ptr(out), _ptr(dots))
     return out, dots
 
 
@@ -778,10 +784,7 @@ def qt_self_attention(qk: torch.Tensor, v: torch.Tensor, num_queries: int, num_h
     M, E2 = qk.shape
     E = E2 // 2
     out = torch.empty(M, E, dtype=torch.float32, device=qk.device)
-    with _call('qt_self_attention', 1):
-        st = lib().cutie_qt_self_attention(_ptr(qk), _ptr(v), _i64(M), _i64(E), ctypes.c_int(num_queries),
-                                           ctypes.c_int(num_heads), _ptr(out), _stream())
-    _check(st, 'cutie_qt_self_attention')
+    _launch('qt_self_attention', 'cutie_qt_self_attention', 1, _ptr(qk), _ptr(v), M, E, num_queries, num_heads, _ptr(out))
     return out
 
 
@@ -796,10 +799,8 @@ def qt_aux_mask(pixel: torch.Tensor, w: torch.Tensor, b: torch.Tensor, B: int, K
     logits = torch.empty(B, K, HW, dtype=torch.float32, device=dev)
     fg = torch.empty(B, K, HW, dtype=torch.uint8, device=dev)
     cnt = torch.zeros(BK, dtype=torch.int32, device=dev)
-    with _call('qt_aux_mask', 1):
-        st = lib().cutie_qt_aux_mask(_ptr(pixel), _ptr(w), _ptr(b), _i64(B), _i64(K), _i64(E), _i64(HW),
-                                     _ptr(logits), _ptr(fg, torch.uint8), _ptr(cnt, torch.int32), _stream())
-    _check(st, 'cutie_qt_aux_mask')
+    _launch('qt_aux_mask', 'cutie_qt_aux_mask', 1, _ptr(pixel), _ptr(w), _ptr(b), B, K, E, HW, _ptr(logits),
+            _ptr(fg, torch.uint8), _ptr(cnt, torch.int32))
     return logits, fg, cnt
 
 
@@ -808,10 +809,7 @@ def qt_mask_logits(pixel: torch.Tensor, w: torch.Tensor, b: torch.Tensor, B: int
     BK, E, HW = pixel.shape
     assert pixel.is_contiguous(), 'pixel must be channel-major contiguous [B*K, E, HW]'
     logits = torch.empty(B, K, HW, dtype=torch.float32, device=pixel.device)
-    with _call('qt_mask_logits', 1):
-        st = lib().cutie_qt_mask_logits(_ptr(pixel), _ptr(w), _ptr(b), _i64(B), _i64(K), _i64(E), _i64(HW),
-                                        _ptr(logits), _stream())
-    _check(st, 'cutie_qt_mask_logits')
+    _launch('qt_mask_logits', 'cutie_qt_mask_logits', 1, _ptr(pixel), _ptr(w), _ptr(b), B, K, E, HW, _ptr(logits))
     return logits
 
 
@@ -823,10 +821,8 @@ def qt_aux_fg(logits: torch.Tensor, positions: torch.Tensor):
     assert logits.is_contiguous() and positions.is_contiguous()
     fg = torch.empty(B, n, HW, dtype=torch.uint8, device=logits.device)
     cnt = torch.zeros(B * n, dtype=torch.int32, device=logits.device)
-    with _call('qt_aux_fg', 1):
-        st = lib().cutie_qt_aux_fg(_ptr(logits), _ptr(positions, torch.int32), _i64(B), _i64(K), _i64(n), _i64(HW),
-                                   _ptr(fg, torch.uint8), _ptr(cnt, torch.int32), _stream())
-    _check(st, 'cutie_qt_aux_fg')
+    _launch('qt_aux_fg', 'cutie_qt_aux_fg', 1, _ptr(logits), _ptr(positions, torch.int32), B, K, n, HW,
+            _ptr(fg, torch.uint8), _ptr(cnt, torch.int32))
     return fg, cnt
 
 
@@ -835,22 +831,21 @@ def qt_pixel_to_query_tiles(qfold: torch.Tensor, pixel: torch.Tensor, pixel_pe: 
     """The tensor-core half of qt_pixel_to_query only: per 64-pixel tile and object the tile-local softmax statistics and
     Z = P . pixel^T go to a workspace; the merge + value projection then runs as QtChain.p2q_combine inside the next fused
     query chain.  Returns (workspace, tiles)."""
-    M, H, E = qfold.shape
+    return _pixel_to_query(qfold, pixel, pixel_pe, fg, fg_count, None, None, None, num_queries, num_heads)
+
+
+def _pixel_to_query(qfold, pixel, pixel_pe, fg, fg_count, wv, bv, out, num_queries, num_heads):
+    """cutie_qt_pixel_to_query: the tile pass alone (wv, bv, out None: 1 launch) or with the combine (2 launches).
+    Returns (workspace, tiles)."""
+    E = qfold.shape[2]
     BK, _, HW = pixel.shape
     assert pixel.is_contiguous() and pixel_pe.is_contiguous() and qfold.is_contiguous() and fg.is_contiguous()
-    L = lib()
-    L.cutie_qt_pixel_to_query_splits.restype = ctypes.c_int
-    L.cutie_qt_pixel_to_query_workspace_floats.restype = ctypes.c_int64
-    splits = L.cutie_qt_pixel_to_query_splits(_i64(BK), _i64(HW), ctypes.c_int(num_heads))
-    ws = torch.empty(int(L.cutie_qt_pixel_to_query_workspace_floats(_i64(BK), _i64(HW))), dtype=torch.float32,
-                     device=pixel.device)
-    with _call('qt_pixel_to_query', 1):
-        st = L.cutie_qt_pixel_to_query(_ptr(qfold), _ptr(pixel), _ptr(pixel_pe), _ptr(fg, torch.uint8),
-                                       _ptr(fg_count, torch.int32), _ptr(None), _i64(0), _ptr(None),
-                                       _i64(BK), _i64(E), _i64(HW), ctypes.c_int(num_queries), ctypes.c_int(num_heads),
-                                       ctypes.c_int(splits), _ptr(ws), _ptr(None), _stream())
-    _check(st, 'cutie_qt_pixel_to_query')
-    return ws, int(splits)
+    splits = _entry('cutie_qt_pixel_to_query_splits')(BK, HW, num_heads)
+    ws = torch.empty(_entry('cutie_qt_pixel_to_query_workspace_floats')(BK, HW), dtype=torch.float32, device=pixel.device)
+    _launch('qt_pixel_to_query', 'cutie_qt_pixel_to_query', 1 if out is None else 2, _ptr(qfold), _ptr(pixel),
+            _ptr(pixel_pe), _ptr(fg, torch.uint8), _ptr(fg_count, torch.int32), _ptr(wv),
+            0 if wv is None else wv.stride(0), _ptr(bv), BK, E, HW, num_queries, num_heads, splits, _ptr(ws), _ptr(out))
+    return ws, splits
 
 
 def qt_pixel_to_query(qfold: torch.Tensor, pixel: torch.Tensor, pixel_pe: torch.Tensor, fg: torch.Tensor,
@@ -863,21 +858,8 @@ def qt_pixel_to_query(qfold: torch.Tensor, pixel: torch.Tensor, pixel_pe: torch.
     Returns attn [M, E] (to be passed through the output projection by qt_linear).  One CTA per 64-pixel tile and
     object (tile-local softmax), then a combine kernel; the tile count is fixed by HW (deterministic)."""
     M, H, E = qfold.shape
-    BK, _, HW = pixel.shape
-    assert pixel.is_contiguous() and pixel_pe.is_contiguous() and qfold.is_contiguous() and fg.is_contiguous()
-    dev = pixel.device
-    out = torch.empty(M, E, dtype=torch.float32, device=dev)
-    L = lib()
-    L.cutie_qt_pixel_to_query_splits.restype = ctypes.c_int
-    L.cutie_qt_pixel_to_query_workspace_floats.restype = ctypes.c_int64
-    splits = L.cutie_qt_pixel_to_query_splits(_i64(BK), _i64(HW), ctypes.c_int(num_heads))
-    ws = torch.empty(int(L.cutie_qt_pixel_to_query_workspace_floats(_i64(BK), _i64(HW))), dtype=torch.float32, device=dev)
-    with _call('qt_pixel_to_query', 2):
-        st = L.cutie_qt_pixel_to_query(_ptr(qfold), _ptr(pixel), _ptr(pixel_pe), _ptr(fg, torch.uint8),
-                                       _ptr(fg_count, torch.int32), _ptr(wv), _i64(wv.stride(0)), _ptr(bv),
-                                       _i64(BK), _i64(E), _i64(HW), ctypes.c_int(num_queries), ctypes.c_int(num_heads),
-                                       ctypes.c_int(splits), _ptr(ws), _ptr(out), _stream())
-    _check(st, 'cutie_qt_pixel_to_query')
+    out = torch.empty(M, E, dtype=torch.float32, device=pixel.device)
+    _pixel_to_query(qfold, pixel, pixel_pe, fg, fg_count, wv, bv, out, num_queries, num_heads)
     return out
 
 
@@ -893,11 +875,8 @@ def qt_query_to_pixel(kfold: torch.Tensor, kdots: torch.Tensor, vfold: torch.Ten
     assert pixel.is_contiguous() and pixel_pe.is_contiguous() and kfold.is_contiguous() and vfold.is_contiguous()
     if out is None:
         out = torch.empty_like(pixel)
-    with _call('qt_query_to_pixel', 1):
-        st = lib().cutie_qt_query_to_pixel(_ptr(kfold), _ptr(kdots), _ptr(vfold), _ptr(out_bias), _ptr(pixel),
-                                           _ptr(pixel_pe), _i64(BK), _i64(E), _i64(HW), ctypes.c_int(num_queries),
-                                           ctypes.c_int(num_heads), _ptr(out), _stream())
-    _check(st, 'cutie_qt_query_to_pixel')
+    _launch('qt_query_to_pixel', 'cutie_qt_query_to_pixel', 1, _ptr(kfold), _ptr(kdots), _ptr(vfold), _ptr(out_bias),
+            _ptr(pixel), _ptr(pixel_pe), BK, E, HW, num_queries, num_heads, _ptr(out))
     return out
 
 
@@ -908,12 +887,6 @@ QT_CHAIN_MAX_OPS = 16
 QT_CHAIN_MAX_TILES = 1024           # pixel tiles the in-chain combine can merge (64 pixels each)
 _QT_LINEAR, _QT_HEAD_FOLD, _QT_SELF_ATTENTION, _QT_P2Q_COMBINE = 0, 1, 2, 3
 _QT_SYNC = {}                        # device index -> 4 x uint32 grid-barrier counters (zero between launches)
-
-
-class _QtOp(ctypes.Structure):       # mirrors `cutie_qt_op` (include/cutie_b200.h)
-    _fields_ = [('kind', ctypes.c_int32), ('phase', ctypes.c_int32), ('inp', ctypes.c_void_p * 8),
-                ('out', ctypes.c_void_p * 2), ('i', ctypes.c_int64 * 6), ('f', ctypes.c_float),
-                ('reserved', ctypes.c_int32)]
 
 
 class QtChain:
@@ -972,10 +945,6 @@ class QtChain:
             qt_chain_run(self)
 
 
-def _vp(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
 def qt_chain_run(chain: QtChain):
     """One cutie_qt_chain launch for the recorded ops."""
     n = len(chain.ops)
@@ -1022,9 +991,5 @@ def qt_chain_run(chain: QtChain):
                               'grid-barrier counters); warm the model up eagerly once')
         sync = _QT_SYNC[dev.index] = torch.zeros(4, dtype=torch.int32, device=dev)
     pf = [w for w in chain.prefetch if w.is_contiguous()][:16]
-    PA, IA = ctypes.c_void_p * max(len(pf), 1), ctypes.c_int64 * max(len(pf), 1)
-    with _call('qt_chain', 1):
-        st = lib().cutie_qt_chain(arr, ctypes.c_int(n), PA(*[w.data_ptr() for w in pf]),
-                                  IA(*[w.numel() * 4 for w in pf]), ctypes.c_int(len(pf)),
-                                  _ptr(sync, torch.int32), _stream())
-    _check(st, 'cutie_qt_chain')
+    _launch('qt_chain', 'cutie_qt_chain', 1, arr, n, _array(ctypes.c_void_p, (w.data_ptr() for w in pf)),
+            _array(ctypes.c_int64, (w.numel() * 4 for w in pf)), len(pf), _ptr(sync, torch.int32))

@@ -222,11 +222,9 @@ def test_lookahead_announced_in_one_mode_misses_in_the_other():
 
 def test_new_entry_points_are_exported_and_validate_on_the_host():
     import __graft_entry__ as ge
+    from cutie_b200 import kernels
     ge.build()
-    lib = ctypes.CDLL(ge.LIB)
-    lib.cutie_b200_last_error.restype = ctypes.c_char_p
-    for f in (lib.cutie_conv_weight_image_f16_bytes, lib.cutie_conv_weight_image_bytes):
-        f.restype = ctypes.c_int64
+    lib = kernels.lib()
     i64 = ctypes.c_int64
     assert lib.cutie_conv_weight_image_f16_bytes(i64(200), i64(64), 3) == 2 * 2 * 9 * 8192
     assert 4 * lib.cutie_conv_weight_image_f16_bytes(i64(256), i64(1024), 1) == lib.cutie_conv_weight_image_bytes(i64(256), i64(1024), 1)

@@ -16,23 +16,23 @@ def _declared():
 
 def test_library_builds_loads_and_exports_header_symbols():
     import __graft_entry__ as ge
+    from cutie_b200 import kernels
     ge.build()
-    lib = ctypes.CDLL(ge.LIB)
+    lib = kernels.lib()
     names = _declared()
     assert len(names) >= 18
     for n in names:
         assert hasattr(lib, n), f'{n} declared in include/cutie_b200.h but not exported'
     assert lib.cutie_b200_abi_version() == 1
-    lib.cutie_b200_last_error.restype = ctypes.c_char_p
     assert lib.cutie_b200_last_error() is not None
 
 
 def test_argument_validation_needs_no_gpu():
     """Invalid arguments are rejected before any CUDA call and set the thread-local error string."""
     import __graft_entry__ as ge
+    from cutie_b200 import kernels
     ge.build()
-    lib = ctypes.CDLL(ge.LIB)
-    lib.cutie_b200_last_error.restype = ctypes.c_char_p
+    lib = kernels.lib()
     st = lib.cutie_obj_summary_accumulate(None, None, ctypes.c_int64(4), None)
     assert st == -1 and b'cutie_obj_summary_accumulate' in lib.cutie_b200_last_error()
     st = lib.cutie_qt_self_attention(None, None, ctypes.c_int64(16), ctypes.c_int64(256), 16, 8, None, None)
@@ -43,10 +43,10 @@ def test_query_chain_op_list_is_validated_on_the_host():
     """cutie_qt_chain checks its op list (counts, phase order, per-kind required pointers and sizes, the two coupled
     optional arguments of each op) before any CUDA call; cutie_consolidate_partial wants both statistics or neither."""
     import __graft_entry__ as ge
+    from cutie_b200 import kernels
     from cutie_b200.kernels import _QtOp
     ge.build()
-    lib = ctypes.CDLL(ge.LIB)
-    lib.cutie_b200_last_error.restype = ctypes.c_char_p
+    lib = kernels.lib()
     sync = (ctypes.c_uint32 * 4)()
     one = ctypes.c_void_p(0x1000)                      # never dereferenced: validation fails first
 
@@ -99,8 +99,9 @@ def test_affinity_plan_is_pure_host_logic():
     """Which passes cutie_affinity_topk runs for a bank size (no GPU needed): exact scan below the threshold,
     nested wgmma filter levels (strides 16^l) above it, coarsest sample never above 4096 tokens."""
     import __graft_entry__ as ge
+    from cutie_b200 import kernels
     ge.build()
-    lib = ctypes.CDLL(ge.LIB)
+    lib = kernels.lib()
     plan = lambda n, k=30: lib.cutie_affinity_plan_levels(ctypes.c_int64(n), k)
     lib.cutie_set_tc_min_tokens(ctypes.c_int64(-1))
     assert plan(100) == 0 and plan(1620) == 0 and plan(4860) == 0

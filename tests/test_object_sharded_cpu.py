@@ -236,9 +236,9 @@ def test_split_aux_entries_validate_arguments_on_the_host():
     any CUDA call."""
     import ctypes
     import __graft_entry__ as ge
+    from cutie_b200 import kernels
     ge.build()
-    lib = ctypes.CDLL(ge.LIB)
-    lib.cutie_b200_last_error.restype = ctypes.c_char_p
+    lib = kernels.lib()
     one = ctypes.c_void_p(0x1000)                      # never dereferenced: validation fails first
     i64 = ctypes.c_int64
     ml = lib.cutie_qt_mask_logits
