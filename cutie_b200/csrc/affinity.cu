@@ -1,5 +1,7 @@
-// Pixel-memory readout for sm_90a: similarity scan + exact streaming top-k, split merge + softmax,
-// sparse value gather.  See include/cutie_b200.h for the contract and DESIGN.md for the roofline.
+// Pixel-memory readout for sm_90a: similarity scan + exact streaming top-k, split merge + softmax, sparse value
+// gather, usage commit; the plan (which passes run for a bank) and the host orchestration of both filtered plans --
+// the TF32 levels of affinity_tc.cu and the FP16 image plan of affinity_f16.cu.  See include/cutie_b200.h for the
+// contract and DESIGN.md for the roofline.
 //
 // Kernel 1  affinity_scan_kernel   grid (query tiles of 64, key splits, B), 256 threads, ~204 KB smem
 //   Streams its split of the memory bank through a 2-stage cp.async pipeline of 128-token tiles
@@ -12,6 +14,7 @@
 //   the winners, optional fixed-point usage accumulation (deterministic).
 // Kernel 3  readout_gather_kernel  one warp per query x object: gathers the k winning 1 KB value rows,
 //   accumulates in registers, transposes through smem to the channel-major [B,K,CV,Q] output.
+// Kernel 4  usage_commit_kernel    use_cnt += the fixed-point usage accumulators, life_cnt += 1.
 #include <stdlib.h>
 
 #include "topk_common.cuh"
@@ -385,7 +388,7 @@ constexpr int TC_CAP = 4096;           // candidate slots per query (also the la
 constexpr int TC_CAP_BIG = 16384;      // slots per query used for the candidate lists (overflow => exhaustive rescan of that query)
 
 static long long g_tc_min_override = -1;
-static long long g_image_level_launches = 0;     // filter levels served from a key image (tests / diagnostics)
+static long long g_image_level_launches = 0;     // calls served by the FP16 image plan (tests / diagnostics)
 
 static long long tc_min_tokens() {
   if (g_tc_min_override >= 0) return g_tc_min_override;
@@ -420,29 +423,69 @@ struct WsLayout {
   size_t total;
 };
 
+// What every plan writes: cutie_affinity_topk's out_idx / out_w and its optional out_sim / usage_acc.
+struct TopkOut {
+  int* idx;
+  float* w;
+  float* sim;
+  unsigned long long* usage_acc;
+};
+
+static size_t ws_take(size_t& off, size_t bytes) {
+  const size_t o = off;
+  off += (bytes + 255) / 256 * 256;
+  return o;
+}
+
+// Workspace of the filtered plans from `off` on: per-query candidate lists, their counters, two threshold buffers.
+static void filtered_ws_layout(WsLayout& w, size_t& off, long long B, long long Q) {
+  w.cand_idx = ws_take(off, (size_t)B * Q * TC_CAP_BIG * 4);
+  w.cand_e = ws_take(off, (size_t)B * Q * TC_CAP_BIG * 4);
+  w.count = ws_take(off, (size_t)B * Q * 4);
+  w.dmax = ws_take(off, (size_t)B * Q * 4);
+  w.emax0 = ws_take(off, (size_t)B * Q * 4);
+  w.emax1 = ws_take(off, (size_t)B * Q * 4);
+}
+
 static WsLayout ws_layout(long long B, long long Q, long long n_total, int top_k) {
   const int kpad = top_k <= 32 ? 32 : 64;
-  const Plan pl = make_plan(n_total, top_k);
   WsLayout w;
   memset(&w, 0, sizeof(w));
   size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-  if (pl.levels == 0) {
-    w.part = take((size_t)B * pick_splits(B, Q, n_total) * Q * kpad * 8);
-  } else {
-    w.cand_idx = take((size_t)B * Q * TC_CAP_BIG * 4);
-    w.cand_e = take((size_t)B * Q * TC_CAP_BIG * 4);
-    w.count = take((size_t)B * Q * 4);
-    w.dmax = take((size_t)B * Q * 4);
-    w.emax0 = take((size_t)B * Q * 4);
-    w.emax1 = take((size_t)B * Q * 4);
-  }
+  if (make_plan(n_total, top_k).levels == 0)
+    w.part = ws_take(off, (size_t)B * pick_splits(B, Q, n_total) * Q * kpad * 8);
+  else
+    filtered_ws_layout(w, off, B, Q);
   w.total = off + 256;
   return w;
 }
 
-static int run_exact(const ScanParams& base, long long B, int nsplit, int* out_idx, float* out_w, float* out_sim,
-                     unsigned long long* usage_acc, cudaStream_t st) {
+// Merge `nsplit` sorted lists per query into the top-k + softmax (topk_merge_kernel).
+static int launch_merge(const float* part_val, const int* part_idx, long long B, long long Q, long long n_total,
+                        int nsplit, int top_k, int kpad, const TopkOut& out, cudaStream_t st) {
+  MergeParams mp;
+  mp.part_val = part_val;
+  mp.part_idx = part_idx;
+  mp.Q = Q;
+  mp.n_total = n_total;
+  mp.nsplit = nsplit;
+  mp.top_k = top_k;
+  mp.kpad = kpad;
+  mp.out_idx = out.idx;
+  mp.out_w = out.w;
+  mp.out_sim = out.sim;
+  mp.usage_acc = out.usage_acc;
+  dim3 mgrid((unsigned)((Q + 7) / 8), (unsigned)B);
+  if (kpad == 32)
+    topk_merge_kernel<1><<<mgrid, 256, 0, st>>>(mp);
+  else
+    topk_merge_kernel<2><<<mgrid, 256, 0, st>>>(mp);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_cuda_error("topk_merge_kernel", e);
+  return 0;
+}
+
+static int run_exact(const ScanParams& base, long long B, int nsplit, const TopkOut& out, cudaStream_t st) {
   ScanParams sp = base;
   const long long ntiles = (sp.samp_count + TK - 1) / TK;
   sp.nsplit = nsplit;
@@ -461,26 +504,7 @@ static int run_exact(const ScanParams& base, long long B, int nsplit, int* out_i
     affinity_scan_kernel<2><<<grid, NT, smem, st>>>(sp);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_cuda_error("affinity_scan_kernel", e);
-  MergeParams mp;
-  mp.part_val = sp.part_val;
-  mp.part_idx = sp.part_idx;
-  mp.Q = sp.Q;
-  mp.n_total = sp.n_total;
-  mp.nsplit = nsplit;
-  mp.top_k = sp.top_k;
-  mp.kpad = sp.kpad;
-  mp.out_idx = out_idx;
-  mp.out_w = out_w;
-  mp.out_sim = out_sim;
-  mp.usage_acc = usage_acc;
-  dim3 mgrid((unsigned)((sp.Q + 7) / 8), (unsigned)B);
-  if (sp.kpad == 32)
-    topk_merge_kernel<1><<<mgrid, 256, 0, st>>>(mp);
-  else
-    topk_merge_kernel<2><<<mgrid, 256, 0, st>>>(mp);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return set_cuda_error("topk_merge_kernel", e);
-  return 0;
+  return launch_merge(sp.part_val, sp.part_idx, B, sp.Q, sp.n_total, nsplit, sp.top_k, sp.kpad, out, st);
 }
 
 // Optional per-phase timing of the filtered plan (diagnostics: bench.py --phase-timing).  Events are recorded on
@@ -509,19 +533,31 @@ static int phase_begin(cudaStream_t st) {
   return slot;
 }
 
-// Optional precomputed operand images of the arenas the segments live in (cutie_bank_key_image).
-struct ImageArgs {
-  bool on;
-  const float* mu;            // [B][64] key centre of the images (null = 0)
-  const int* seed_idx;        // [B][Q][kpad] threshold seeds (null = none)
-  const float* img[kMaxSeg];
-  long long bs[kMaxSeg];      // batch stride (floats)
-  long long phys[kMaxSeg];    // physical index of the segment's first token inside its arena
-};
+// Exact re-rank of the candidate lists a filtered plan left in the workspace (affinity_rerank_kernel).
+static int rerank_candidates(const ScanParams& base, long long B, char* ws, const WsLayout& wl, const TopkOut& out,
+                             cudaStream_t st) {
+  RerankParams rp;
+  memset(&rp, 0, sizeof(rp));
+  rp.segs = base.segs;
+  rp.qk = base.qk;
+  rp.qe = base.qe;
+  rp.Q = base.Q;
+  rp.n_total = base.n_total;
+  rp.cand_idx = (const int*)(ws + wl.cand_idx);
+  rp.count = (const int*)(ws + wl.count);
+  rp.cap = TC_CAP_BIG;
+  rp.top_k = base.top_k;
+  rp.kpad = base.kpad;
+  rp.out_idx = out.idx;
+  rp.out_w = out.w;
+  rp.out_sim = out.sim;
+  rp.usage_acc = out.usage_acc;
+  return launch_rerank(rp, B, st);
+}
 
 // One filter level: zero the per-query counters, wgmma filter over the stride-`stride` sample.
 static int run_filter_level(const ScanParams& base, long long B, long long stride, const float* emax_in, char* ws,
-                            const WsLayout& wl, float* dbg_energy, const ImageArgs& ia, cudaStream_t st) {
+                            const WsLayout& wl, float* dbg_energy, cudaStream_t st) {
   TcFilterParams fp;
   memset(&fp, 0, sizeof(fp));
   fp.segs = base.segs;
@@ -541,69 +577,60 @@ static int run_filter_level(const ScanParams& base, long long B, long long strid
   fp.dmax = (float*)(ws + wl.dmax);
   fp.cap = TC_CAP_BIG;
   fp.dbg_energy = dbg_energy;
-  if (ia.on && stride == 1 && emax_in != nullptr) {
-    // the whole bank, one bulk copy per physical 128-token tile of each segment's arena
-    fp.use_img = 1;
-    static int chunks = -1, prefetch = -1;
-    if (chunks < 0) {
-      const char* e = getenv("CUTIE_B200_IMG_CHUNKS");
-      chunks = e ? atoi(e) : 1;        // measured at cfg 2: 1 x 68 KB and 17 x 4 KB copies per tile are within noise
-      if (chunks < 1 || 69632 % chunks != 0 || (69632 / chunks) % 16 != 0) chunks = 1;
-      const char* f = getenv("CUTIE_B200_IMG_PREFETCH");
-      prefetch = f ? atoi(f) : 0;      // ... and so is an explicit L2 prefetch two tiles ahead
-      if (prefetch < 0 || prefetch > 64) prefetch = 0;
-    }
-    fp.img_chunks = chunks;
-    fp.img_prefetch = prefetch;
-    long long cum = 0;
-    for (int s = 0; s < base.segs.nseg; ++s) {
-      const long long n = base.segs.begin[s + 1] - base.segs.begin[s];
-      fp.img[s] = ia.img[s];
-      fp.img_bs[s] = ia.bs[s];
-      fp.img_tile0[s] = ia.phys[s] / 128;
-      fp.img_lo0[s] = (int)(ia.phys[s] % 128);
-      fp.img_tcum[s] = cum;
-      cum += n > 0 ? (fp.img_lo0[s] + n + 127) / 128 : 0;
-    }
-    for (int s = base.segs.nseg; s <= kMaxSeg; ++s) fp.img_tcum[s] = cum;
-    fp.nsplit = tc_split_count(B, base.Q, cum * 128);
-    fp.tiles_per_split = (int)((cum + fp.nsplit - 1) / fp.nsplit);
-    ++g_image_level_launches;
-  }
   cudaError_t e = cudaMemsetAsync(ws + wl.count, 0, (size_t)(wl.emax0 - wl.count), st);   // count + dmax
   if (e != cudaSuccess) return set_cuda_error("cudaMemsetAsync", e);
   return launch_tc_filter(fp, B, st);
 }
 
+// Where the image tiles of the bank `segs` are, from the caller's per-segment images (cutie_affinity_topk_img:
+// seg_image_bstride in floats, seg_phys_begin = index of the segment's first token inside its arena).  Returns 1 when
+// every non-empty segment has an image (the FP16 plan can run), 0 when one has none (the TF32 levels convert the keys
+// on the fly), < 0 for an invalid argument, reported under the name `fn`.
+static int image_tiles(ImageTiles& t, const KeySegments& segs, const void* const* seg_key_image,
+                       const int64_t* seg_image_bstride, const int64_t* seg_phys_begin, const char* fn) {
+  memset(&t, 0, sizeof(t));
+  if (!seg_key_image) return 0;
+  if (!seg_image_bstride || !seg_phys_begin)
+    return fail(-1, "%s: invalid argument: image strides / physical offsets missing", fn);
+  int on = 1;
+  long long cum = 0;
+  for (int s = 0; s < segs.nseg; ++s) {
+    const long long n = segs.begin[s + 1] - segs.begin[s];
+    if (n > 0 && !seg_key_image[s]) on = 0;
+    if (seg_phys_begin[s] < 0) return fail(-1, "%s: invalid argument: negative physical offset", fn);
+    if (((uintptr_t)seg_key_image[s] & 15) != 0)
+      return fail(-1, "%s: invalid argument: key image must be 16-byte aligned", fn);
+    t.img[s] = (const unsigned char*)seg_key_image[s];
+    t.bs[s] = seg_image_bstride[s] * 4;
+    t.tile0[s] = seg_phys_begin[s] / 128;
+    t.lo0[s] = (int)(seg_phys_begin[s] % 128);
+    t.tcum[s] = cum;
+    cum += n > 0 ? (t.lo0[s] + n + 127) / 128 : 0;
+  }
+  for (int s = segs.nseg; s <= kMaxSeg; ++s) t.tcum[s] = cum;
+  return on;
+}
+
 // FP16 plan over the key operand image: tile-sampled threshold pass -> k-th smallest slot minimum -> candidate filter
 // over the whole image -> exact re-rank.  Two memsets + four launches per call, whatever the bank size.
-static int run_filtered_f16(const ScanParams& base, long long B, char* ws, const WsLayout& wl, int* out_idx, float* out_w,
-                            float* out_sim, unsigned long long* usage_acc, const ImageArgs& ia, cudaStream_t st) {
+// key_mu [B][64]: the key centre of the images (null = 0); seed_idx [B][Q][kpad]: threshold seeds (null = none).
+static int run_filtered_f16(const ScanParams& base, long long B, const ImageTiles& tiles, const float* key_mu,
+                            const int* seed_idx, char* ws, const WsLayout& wl, const TopkOut& out, cudaStream_t st) {
   F16FilterParams fp;
   memset(&fp, 0, sizeof(fp));
   fp.segs = base.segs;
   fp.qk = base.qk;
   fp.qe = base.qe;
-  fp.key_mu = ia.mu;
+  fp.key_mu = key_mu;
   fp.Q = base.Q;
-  long long cum = 0;
-  for (int s = 0; s < base.segs.nseg; ++s) {
-    const long long n = base.segs.begin[s + 1] - base.segs.begin[s];
-    fp.img[s] = reinterpret_cast<const unsigned char*>(ia.img[s]);
-    fp.img_bs[s] = ia.bs[s] * 4;
-    fp.img_tile0[s] = ia.phys[s] / 128;
-    fp.img_lo0[s] = (int)(ia.phys[s] % 128);
-    fp.img_tcum[s] = cum;
-    cum += n > 0 ? (fp.img_lo0[s] + n + 127) / 128 : 0;
-  }
-  for (int s = base.segs.nseg; s <= kMaxSeg; ++s) fp.img_tcum[s] = cum;
+  fp.tiles = tiles;
   const int grid_x = f16_schedule(fp, B);
   const int groups = (fp.full_groups > 0 ? fp.splits_full : fp.splits_half) * 2 * F16_SLOTS;    // threshold slots per query
   if (groups > TC_CAP_BIG) return fail(-1, "%s: too many key splits for the threshold workspace", "run_filtered_f16");
   // sample every `stride`-th tile: every split of a query group should still see >= 8 tiles (its 64 slots then hold
   // minima over >= 16 tokens each); small banks are sampled whole
   const long long max_splits = fp.full_groups > 0 ? fp.splits_full : fp.splits_half;
-  long long stride = cum / (8ll * max_splits);
+  long long stride = tiles.tcum[base.segs.nseg] / (8ll * max_splits);
   if (stride > 8) stride = 8;
   if (stride < 1) stride = 1;
   const int ph = phase_begin(st);
@@ -627,7 +654,7 @@ static int run_filtered_f16(const ScanParams& base, long long B, char* ws, const
   tp.Q = base.Q;
   tp.n_total = base.n_total;
   tp.emax_out = emax;
-  tp.seed_idx = ia.seed_idx;
+  tp.seed_idx = seed_idx;
   tp.segs = base.segs;
   tp.qk = base.qk;
   tp.qe = base.qe;
@@ -644,36 +671,20 @@ static int run_filtered_f16(const ScanParams& base, long long B, char* ws, const
   if (rc) return rc;
   ++g_image_level_launches;
   phase_mark(ph, st);
-  RerankParams rp;
-  memset(&rp, 0, sizeof(rp));
-  rp.segs = base.segs;
-  rp.qk = base.qk;
-  rp.qe = base.qe;
-  rp.Q = base.Q;
-  rp.n_total = base.n_total;
-  rp.cand_idx = (const int*)(ws + wl.cand_idx);
-  rp.count = (const int*)(ws + wl.count);
-  rp.cap = TC_CAP_BIG;
-  rp.top_k = base.top_k;
-  rp.kpad = base.kpad;
-  rp.out_idx = out_idx;
-  rp.out_w = out_w;
-  rp.out_sim = out_sim;
-  rp.usage_acc = usage_acc;
-  rc = launch_rerank(rp, B, st);
+  rc = rerank_candidates(base, B, ws, wl, out, st);
   phase_mark(ph, st);
   return rc;
 }
 
+// TF32 plan: the filter levels, coarsest first, each handing its thresholds to the next -> exact re-rank.
 static int run_filtered(const ScanParams& base, long long B, const Plan& pl, char* ws, const WsLayout& wl,
-                        int* out_idx, float* out_w, float* out_sim, unsigned long long* usage_acc,
-                        float* dbg_energy, const ImageArgs& ia, cudaStream_t st) {
+                        const TopkOut& out, float* dbg_energy, cudaStream_t st) {
   float* emax[2] = {(float*)(ws + wl.emax0), (float*)(ws + wl.emax1)};
   const float* emax_in = nullptr;
   const int ph = phase_begin(st);
   for (int l = 0; l < pl.levels; ++l) {
     const bool last = (l == pl.levels - 1);
-    int rc = run_filter_level(base, B, pl.stride[l], emax_in, ws, wl, last ? dbg_energy : nullptr, ia, st);
+    int rc = run_filter_level(base, B, pl.stride[l], emax_in, ws, wl, last ? dbg_energy : nullptr, st);
     if (rc) return rc;
     phase_mark(ph, st);
     if (!last) {
@@ -691,23 +702,7 @@ static int run_filtered(const ScanParams& base, long long B, const Plan& pl, cha
       emax_in = emax[l & 1];
     }
   }
-  RerankParams rp;
-  memset(&rp, 0, sizeof(rp));
-  rp.segs = base.segs;
-  rp.qk = base.qk;
-  rp.qe = base.qe;
-  rp.Q = base.Q;
-  rp.n_total = base.n_total;
-  rp.cand_idx = (const int*)(ws + wl.cand_idx);
-  rp.count = (const int*)(ws + wl.count);
-  rp.cap = TC_CAP_BIG;
-  rp.top_k = base.top_k;
-  rp.kpad = base.kpad;
-  rp.out_idx = out_idx;
-  rp.out_w = out_w;
-  rp.out_sim = out_sim;
-  rp.usage_acc = usage_acc;
-  const int rc = launch_rerank(rp, B, st);
+  const int rc = rerank_candidates(base, B, ws, wl, out, st);
   phase_mark(ph, st);
   return rc;
 }
@@ -743,7 +738,7 @@ extern "C" int cutie_debug_phase_times(int64_t calls_ago, float* out_ms, int max
   return k;
 }
 
-// How many filter levels have been served from a key image so far in this process (diagnostics / tests).
+// How many calls the FP16 image plan has served so far in this process (diagnostics / tests).
 extern "C" int64_t cutie_debug_image_level_launches(void) { return g_image_level_launches; }
 
 // Which plan cutie_affinity_topk will use: 0 = exact scan only, n >= 1 = n wgmma filter levels (see make_plan).
@@ -803,31 +798,19 @@ extern "C" int cutie_affinity_topk_img(int num_segments, const void* const* seg_
   CUTIE_REQUIRE(workspace_bytes >= wl.total, "workspace too small");
   char* ws = (char*)workspace;
   cudaStream_t st = (cudaStream_t)stream;
+  const TopkOut out = {out_idx, out_w, out_sim, usage_acc};
   const Plan pl = make_plan(n_total, top_k);
   if (pl.levels == 0) {
     const int ns0 = pick_splits(B, Q, n_total);
     sp.part_val = (float*)(ws + wl.part);
     sp.part_idx = (int*)(ws + wl.part + (size_t)B * ns0 * Q * kpad * 4);
-    return run_exact(sp, B, ns0, out_idx, out_w, out_sim, usage_acc, st);
+    return run_exact(sp, B, ns0, out, st);
   }
-  ImageArgs ia;
-  memset(&ia, 0, sizeof(ia));
-  if (seg_key_image) {
-    CUTIE_REQUIRE(seg_image_bstride && seg_phys_begin, "image strides / physical offsets missing");
-    ia.on = true;
-    ia.mu = key_mu;
-    ia.seed_idx = seed_idx;
-    for (int s = 0; s < num_segments; ++s) {
-      if (seg_len[s] > 0 && !seg_key_image[s]) ia.on = false;          // a segment without an image: convert on the fly
-      CUTIE_REQUIRE(seg_phys_begin[s] >= 0, "negative physical offset");
-      CUTIE_REQUIRE(((uintptr_t)seg_key_image[s] & 15) == 0, "key image must be 16-byte aligned");
-      ia.img[s] = (const float*)seg_key_image[s];
-      ia.bs[s] = seg_image_bstride[s];
-      ia.phys[s] = seg_phys_begin[s];
-    }
-  }
-  if (ia.on) return run_filtered_f16(sp, B, ws, wl, out_idx, out_w, out_sim, usage_acc, ia, st);
-  return run_filtered(sp, B, pl, ws, wl, out_idx, out_w, out_sim, usage_acc, nullptr, ia, st);
+  ImageTiles tiles;
+  const int with_images = image_tiles(tiles, sp.segs, seg_key_image, seg_image_bstride, seg_phys_begin, __func__);
+  if (with_images < 0) return with_images;
+  if (with_images) return run_filtered_f16(sp, B, tiles, key_mu, seed_idx, ws, wl, out, st);
+  return run_filtered(sp, B, pl, ws, wl, out, nullptr, st);
 }
 
 extern "C" int cutie_affinity_topk(int num_segments, const void* const* seg_key, const void* const* seg_shrinkage,
@@ -858,23 +841,15 @@ extern "C" int cutie_debug_tc_energy(int num_segments, const void* const* seg_ke
   WsLayout wl;
   memset(&wl, 0, sizeof(wl));
   size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-  wl.cand_idx = take((size_t)B * Q * TC_CAP_BIG * 4);
-  wl.cand_e = take((size_t)B * Q * TC_CAP_BIG * 4);
-  wl.count = take((size_t)B * Q * 4);
-  wl.dmax = take((size_t)B * Q * 4);
-  wl.emax0 = take((size_t)B * Q * 4);
-  wl.emax1 = take((size_t)B * Q * 4);
-  const size_t o_idx = take((size_t)B * Q * 32 * 4), o_w = take((size_t)B * Q * 32 * 4);
+  filtered_ws_layout(wl, off, B, Q);
+  const size_t o_idx = ws_take(off, (size_t)B * Q * 32 * 4), o_w = ws_take(off, (size_t)B * Q * 32 * 4);   // unused outputs
   CUTIE_REQUIRE(workspace_bytes >= off, "workspace too small");
   Plan pl;
   pl.levels = 1;
   pl.stride[0] = 1;
   char* ws = (char*)workspace;
-  ImageArgs ia;
-  memset(&ia, 0, sizeof(ia));
-  return run_filtered(sp, B, pl, ws, wl, (int*)(ws + o_idx), (float*)(ws + o_w), nullptr, nullptr, dbg_energy, ia,
-                      (cudaStream_t)stream);
+  const TopkOut out = {(int*)(ws + o_idx), (float*)(ws + o_w), nullptr, nullptr};
+  return run_filtered(sp, B, pl, ws, wl, out, dbg_energy, (cudaStream_t)stream);
 }
 
 extern "C" int cutie_topk_merge(const float* part_val, const int32_t* part_idx, int64_t B, int64_t nparts, int64_t Q,
@@ -883,25 +858,8 @@ extern "C" int cutie_topk_merge(const float* part_val, const int32_t* part_idx, 
   CUTIE_REQUIRE(part_val && part_idx && out_idx && out_w, "null argument");
   CUTIE_REQUIRE(kpad == 32 || kpad == 64, "kpad must be 32 or 64");
   CUTIE_REQUIRE(top_k >= 1 && top_k <= kpad && nparts >= 1 && B >= 1 && Q >= 1, "bad sizes");
-  MergeParams mp;
-  mp.part_val = part_val;
-  mp.part_idx = part_idx;
-  mp.Q = Q;
-  mp.n_total = n_total;
-  mp.nsplit = (int)nparts;
-  mp.top_k = top_k;
-  mp.kpad = kpad;
-  mp.out_idx = out_idx;
-  mp.out_w = out_w;
-  mp.out_sim = out_sim;
-  mp.usage_acc = usage_acc;
-  dim3 mgrid((unsigned)((Q + 7) / 8), (unsigned)B);
-  if (kpad == 32)
-    topk_merge_kernel<1><<<mgrid, 256, 0, (cudaStream_t)stream>>>(mp);
-  else
-    topk_merge_kernel<2><<<mgrid, 256, 0, (cudaStream_t)stream>>>(mp);
-  CUTIE_CHECK_LAUNCH();
-  return 0;
+  const TopkOut out = {out_idx, out_w, out_sim, usage_acc};
+  return launch_merge(part_val, part_idx, B, Q, n_total, (int)nparts, top_k, kpad, out, (cudaStream_t)stream);
 }
 
 extern "C" int cutie_readout_gather(const int32_t* idx, const float* w, int64_t B, int64_t Q, int kpad,

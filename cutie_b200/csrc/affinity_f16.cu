@@ -51,16 +51,16 @@ __device__ __forceinline__ F16Tile f16_tile(const F16FilterParams& p, int b, lon
   int s = 0;
 #pragma unroll
   for (int i = 1; i < kMaxSeg; ++i)
-    if (i < p.segs.nseg && g >= p.img_tcum[i]) s = i;
-  const long long j = g - p.img_tcum[s];
+    if (i < p.segs.nseg && g >= p.tiles.tcum[i]) s = i;
+  const long long j = g - p.tiles.tcum[s];
   const long long n = p.segs.begin[s + 1] - p.segs.begin[s];
-  const long long lo0 = p.img_lo0[s];
+  const long long lo0 = p.tiles.lo0[s];
   const long long a = lo0 - j * F16_KTILE, e = lo0 + n - j * F16_KTILE;
   F16Tile t;
   t.lo = a < 0 ? 0 : (int)a;
   t.hi = e > F16_KTILE ? F16_KTILE : (int)e;
   t.lbase = p.segs.begin[s] - lo0 + j * F16_KTILE;
-  t.src = p.img[s] + (long long)b * p.img_bs[s] + (p.img_tile0[s] + j) * (long long)F16_OPER_BYTES;
+  t.src = p.tiles.img[s] + (long long)b * p.tiles.bs[s] + (p.tiles.tile0[s] + j) * (long long)F16_OPER_BYTES;
   return t;
 }
 __device__ __forceinline__ unsigned range_mask32(int a, int b) {      // bits [a, b) of a 32-bit word (any ints)
@@ -102,7 +102,7 @@ __global__ void __launch_bounds__(F16_THREADS, 1) affinity_f16_filter_kernel(con
   const long long q0 = (long long)grp * F16_QT;
   const int halves = (q0 + 128 < p.Q) ? 2 : 1;
   // tiles of this CTA: physical image tiles g (SAMPLE: only g = phase + j * stride), dealt round-robin to the splits
-  const long long all_tiles = p.img_tcum[p.segs.nseg];
+  const long long all_tiles = p.tiles.tcum[p.segs.nseg];
   const long long my_pool = SAMPLE ? (all_tiles > p.tile_phase ? (all_tiles - p.tile_phase + p.tile_stride - 1) / p.tile_stride : 0)
                                    : all_tiles;
   const int ntiles = split < my_pool ? (int)((my_pool - split + nsplit - 1) / nsplit) : 0;
@@ -377,7 +377,7 @@ int f16_schedule(F16FilterParams& p, long long B) {
   long long u = sms / (units * B);
   if (u < 1) u = 1;
   if (u > 16) u = 16;                              // 2u splits x 16 threshold slots <= 512 (f16_threshold_kernel)
-  const long long tiles = p.img_tcum[p.segs.nseg];
+  const long long tiles = p.tiles.tcum[p.segs.nseg];
   if (2 * u > tiles) u = (tiles + 1) / 2 > 0 ? (tiles + 1) / 2 : 1;
   p.splits_full = (int)(2 * u);
   p.splits_half = half_groups ? (int)u : 0;

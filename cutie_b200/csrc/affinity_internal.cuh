@@ -1,5 +1,6 @@
-// Internal (non-ABI) interfaces between affinity.cu (exact scan, orchestration) and affinity_tc.cu
-// (wgmma candidate filter, level threshold hand-over, exact re-rank).
+// Internal (non-ABI) interfaces between affinity.cu (exact scan, orchestration of both filtered plans), affinity_tc.cu
+// (TF32 wgmma candidate filter, level threshold hand-over, exact re-rank) and affinity_f16.cu (FP16 wgmma filter over the
+// key operand image, threshold select).
 #pragma once
 #include "common.cuh"
 
@@ -22,16 +23,6 @@ struct TcFilterParams {
   float* dmax;             // [B][Q] largest error bound used (atomicMax on the bit pattern); zeroed by the caller
   int cap;
   float* dbg_energy;       // optional [B][Q][samp_count] tf32 energies (tests)
-  // Image path (stride-1 level only): per segment the precomputed operand image of the arena it lives in
-  // (cutie_bank_key_image), addressed by physical 128-token tile.
-  int use_img;
-  int img_chunks;                  // bulk copies per 68 KB tile (69632 / chunks must be a multiple of 16)
-  int img_prefetch;                // L2 prefetch distance in tiles (0 = off)
-  const float* img[kMaxSeg];
-  long long img_bs[kMaxSeg];       // batch stride (floats)
-  long long img_tile0[kMaxSeg];    // first physical tile of the segment
-  int img_lo0[kMaxSeg];            // row of the segment's first token inside that tile
-  long long img_tcum[kMaxSeg + 1]; // prefix sums of the segments' tile counts
 };
 
 struct SelectParams {
@@ -57,6 +48,16 @@ struct RerankParams {
   unsigned long long* usage_acc;
 };
 
+// Where the image tiles of a bank are: per segment the FP16 operand image of the arena it lives in
+// (cutie_bank_key_image), addressed by physical 128-token tile.
+struct ImageTiles {
+  const unsigned char* img[kMaxSeg];
+  long long bs[kMaxSeg];           // batch stride (bytes)
+  long long tile0[kMaxSeg];        // first physical tile of the segment
+  int lo0[kMaxSeg];                // row of the segment's first token inside that tile
+  long long tcum[kMaxSeg + 1];     // prefix sums of the segments' tile counts
+};
+
 // FP16 filter over the key operand image (affinity_f16.cu): threshold sampling pass + candidate filter pass.
 constexpr int F16_RESERVE = 16;            // candidate slots reserved per global atomic (per thread)
 constexpr int F16_SLOTS = 8;               // running minima per sampling thread (threshold slots = splits x 2 x F16_SLOTS)
@@ -77,12 +78,7 @@ struct F16FilterParams {
   int cap;
   // CTA schedule (f16_schedule)
   int full_groups, splits_full, splits_half;
-  // per segment: the FP16 operand image of the arena it lives in (cutie_bank_key_image), by physical 128-token tile
-  const unsigned char* img[kMaxSeg];
-  long long img_bs[kMaxSeg];       // batch stride (bytes)
-  long long img_tile0[kMaxSeg];    // first physical tile of the segment
-  int img_lo0[kMaxSeg];            // row of the segment's first token inside that tile
-  long long img_tcum[kMaxSeg + 1]; // prefix sums of the segments' tile counts
+  ImageTiles tiles;
 };
 size_t f16_filter_smem_bytes();
 int f16_schedule(F16FilterParams& p, long long B);

@@ -32,45 +32,14 @@ constexpr int QT = TC_QT;               // queries per CTA (MMA M)
 constexpr int KTILE = TC_KTILE;         // memory tokens per tile (MMA N)
 constexpr int BLK_BYTES = TC_BLK_BYTES;
 constexpr int OPER_BYTES = TC_OPER_BYTES;
-// Warp roles.  On-the-fly producers (strided levels): warps 0-3 MMA + epilogue, 4-11 two producer groups = 384
-// threads.  Image path: the producer is ONE thread issuing bulk copies, so the freed warps become MMA + epilogue
-// warpgroups -- warps 0-15 (warpgroup = warp >> 2 = its 32-column group: four warpgroups hide each other's MMA /
-// select latency), warp 16 bulk-copy producer = 544 threads.
-constexpr int TC_THREADS = 384;
-constexpr int TC_THREADS_IMG = 544;
+constexpr int TC_THREADS = 384;         // warps 0-3 MMA + epilogue, warps 4-11 two producer groups
 constexpr float TF32_EPS = TC_TF32_EPS;
 
 // K-major un-swizzled descriptor of the [128 x 32 B] tail block: chunk-major, 16 row-groups of chunk 0 (128 B each),
 // then chunk 1 at +2048 B.
 __device__ __forceinline__ uint64_t desc_tail(uint32_t addr) { return desc_interleave(addr, 2048, 128); }
-// Bulk-copy path (IMG): tiles are the bank's precomputed operand image (cutie_bank_key_image), addressed by PHYSICAL
-// 128-token tile of the arena each segment lives in; rows outside the segment are masked in the epilogue.
-struct ImgTile {
-  const unsigned char* src;   // 69632 contiguous bytes: the tile exactly as the MMA wants it in shared memory
-  int lo, hi;                 // rows [lo, hi) of the tile belong to the segment
-  long long lbase;            // bank (logical) index of row 0
-};
-__device__ __forceinline__ ImgTile img_tile(const TcFilterParams& p, int b, long long g) {
-  int s = 0;
-#pragma unroll
-  for (int i = 1; i < kMaxSeg; ++i)
-    if (i < p.segs.nseg && g >= p.img_tcum[i]) s = i;
-  const long long j = g - p.img_tcum[s];
-  const long long n = p.segs.begin[s + 1] - p.segs.begin[s];
-  const long long lo0 = p.img_lo0[s];
-  const long long a = lo0 - j * KTILE, e = lo0 + n - j * KTILE;
-  ImgTile t;
-  t.lo = a < 0 ? 0 : (int)a;
-  t.hi = e > KTILE ? KTILE : (int)e;
-  t.lbase = p.segs.begin[s] - lo0 + j * KTILE;
-  t.src = reinterpret_cast<const unsigned char*>(p.img[s] + (long long)b * p.img_bs[s]) +
-          (p.img_tile0[s] + j) * (long long)OPER_BYTES;
-  return t;
-}
-__device__ __forceinline__ unsigned range_mask32(int a, int b) {      // bits [a, b) of a 32-bit word (any ints)
-  const unsigned hi = b >= 32 ? 0xffffffffu : (b <= 0 ? 0u : ((1u << b) - 1u));
-  const unsigned lo = a <= 0 ? 0xffffffffu : (a >= 32 ? 0u : ~((1u << a) - 1u));
-  return hi & lo;
+__device__ __forceinline__ unsigned low_mask32(int n) {      // bits [0, n) of a 32-bit word (any int)
+  return n >= 32 ? 0xffffffffu : (n <= 0 ? 0u : ((1u << n) - 1u));
 }
 struct TcSmemTail {
   unsigned long long full[2], empty[2];
@@ -79,10 +48,10 @@ struct TcSmemTail {
   float vq[QT];              // [query row] sqrt(b2)
 };
 
-template <bool DBG, bool IMG>
-__global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity_tc_filter_kernel(const TcFilterParams p) {
-  constexpr int EPI_WARPS = IMG ? 16 : 4;
-  constexpr int RESERVE = IMG ? 16 : 32;     // candidate slots reserved per global atomic (per thread)
+template <bool DBG>
+__global__ void __launch_bounds__(TC_THREADS, 1) affinity_tc_filter_kernel(const TcFilterParams p) {
+  constexpr int EPI_WARPS = 4;
+  constexpr int RESERVE = 32;     // candidate slots reserved per global atomic (per thread)
   extern __shared__ __align__(1024) unsigned char smem[];
   unsigned char* A = smem;                              // queries
   unsigned char* Bst = smem + OPER_BYTES;               // 2 stages of keys
@@ -93,8 +62,8 @@ __global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity
   // Tiles are dealt to the key splits round-robin (split s takes tiles s, s + nsplit, ...): candidates cluster in
   // the part of the bank that resembles the current frame (recent memory frames), and contiguous ranges would
   // leave the CTAs owning that part with nearly all of the candidate work.
-  // non-IMG: tile g covers sample indices [128 g, 128 g + 128); IMG: g enumerates the segments' physical image tiles
-  const long long total_tiles = IMG ? p.img_tcum[p.segs.nseg] : (p.samp_count + KTILE - 1) / KTILE;
+  // Tile g covers sample indices [128 g, 128 g + 128).
+  const long long total_tiles = (p.samp_count + KTILE - 1) / KTILE;
   const long long tile_step = p.nsplit;
   const long long i_end = p.samp_count;
   const int ntiles = split < total_tiles ? (int)((total_tiles - split + tile_step - 1) / tile_step) : 0;
@@ -102,7 +71,7 @@ __global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity
 
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&T.full[s]), IMG ? 1 : 128);   // IMG: one arrive.expect_tx + the bulk copy's bytes
+      mbar_init(smem_u32(&T.full[s]), 128);               // every thread of the producer group that converted the tile
       mbar_init(smem_u32(&T.empty[s]), 32 * EPI_WARPS);   // every MMA + epilogue thread is done with the tile
     }
     mbar_init_fence();
@@ -143,7 +112,7 @@ __global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity
   __syncthreads();
 
   if (warp < EPI_WARPS) {
-    // =========================== epilogue: thread == query (x column group on the image path) ===========================
+    // =========================== epilogue: thread == query ===========================
     const int row = frag_row(warp & 3, lane);                // the query row frag_rows32 gives this thread
     const long long q = q0 + row;
     const float vq = T.vq[row];
@@ -161,16 +130,10 @@ __global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity
       mbar_wait(smem_u32(&T.full[a]), (t >> 1) & 1);
       const uint32_t b_base = smem_u32(Bst + a * OPER_BYTES);
       const float thr = (q < p.Q) ? emax : -CUDART_INF_F;
-      long long ibase = tile_of(t) * KTILE;                  // IMG: bank index of row 0 (may precede the segment)
-      int vlo = 0, nvalid = (int)((i_end - ibase) < KTILE ? (i_end - ibase) : KTILE);   // valid rows [vlo, nvalid)
-      if (IMG) {
-        const ImgTile it = img_tile(p, b, tile_of(t));
-        ibase = it.lbase;
-        vlo = it.lo;
-        nvalid = it.hi;
-      }
+      const long long ibase = tile_of(t) * KTILE;
+      const int nvalid = (int)((i_end - ibase) < KTILE ? (i_end - ibase) : KTILE);      // valid rows [0, nvalid)
 #pragma unroll 1
-      for (int cg = IMG ? (warp >> 2) : 0; cg < (IMG ? (warp >> 2) + 1 : 4); ++cg) {
+      for (int cg = 0; cg < 4; ++cg) {
         // D[128 queries x 32 tokens of group cg] as two M = 64 halves, K = 4 x 32 (swizzled blocks) + 8 (tail)
         float d0[16], d1[16];
         wg_fence_acc(d0);
@@ -198,38 +161,35 @@ __global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity
         if (DBG) {
           if (q < p.Q)
             for (int j = 0; j < 32; ++j)
-              if (cg * 32 + j >= vlo && cg * 32 + j < nvalid && ibase + cg * 32 + j < p.samp_count)
+              if (cg * 32 + j < nvalid && ibase + cg * 32 + j < p.samp_count)
                 p.dbg_energy[((long long)b * p.Q + q) * p.samp_count + ibase + cg * 32 + j] = __uint_as_float(r[j]);
         }
         // branch-free per-lane bitmask of passing columns (2 instructions per element) ...
         unsigned mask = 0u;
 #pragma unroll
         for (int j = 0; j < 32; ++j) mask |= (__uint_as_float(r[j]) < thr) ? (1u << j) : 0u;
-        mask &= range_mask32(vlo - cg * 32, nvalid - cg * 32);   // columns of this group that hold real tokens
+        mask &= low_mask32(nvalid - cg * 32);                    // columns of this group that hold real tokens
         // ... and a per-lane walk over the lane's own passing columns (iterations per group = the largest popcount
-        // among the 32 queries, not the number of distinct passing columns).  Strided levels also need the value: it
+        // among the 32 queries, not the number of distinct passing columns).  The threshold hand-over also needs the value: it
         // is picked out of the 32 registers with a 5-level select tree on the column bits (31 SEL; no accumulator re-read,
-        // no dynamic register indexing).  The image path keeps only the index -- its survivors are re-ranked exactly.
+        // no dynamic register indexing).
         unsigned m = mask;
         while (m) {
           const int j = __ffs(m) - 1;
           m &= m - 1;
           const int col = cg * 32 + j;
-          float e_hi = 0.f;
-          if (!IMG) {
-            uint32_t s16[16], s8[8], s4[4];
-            const bool b4 = (j & 16) != 0, b3 = (j & 8) != 0, b2 = (j & 4) != 0, b1 = (j & 2) != 0, b0 = (j & 1) != 0;
+          uint32_t s16[16], s8[8], s4[4];
+          const bool b4 = (j & 16) != 0, b3 = (j & 8) != 0, b2 = (j & 4) != 0, b1 = (j & 2) != 0, b0 = (j & 1) != 0;
 #pragma unroll
-            for (int i = 0; i < 16; ++i) s16[i] = b4 ? r[16 + i] : r[i];
+          for (int i = 0; i < 16; ++i) s16[i] = b4 ? r[16 + i] : r[i];
 #pragma unroll
-            for (int i = 0; i < 8; ++i) s8[i] = b3 ? s16[8 + i] : s16[i];
+          for (int i = 0; i < 8; ++i) s8[i] = b3 ? s16[8 + i] : s16[i];
 #pragma unroll
-            for (int i = 0; i < 4; ++i) s4[i] = b2 ? s8[4 + i] : s8[i];
-            const uint32_t s2a = b1 ? s4[2] : s4[0], s2b = b1 ? s4[3] : s4[1];
-            const float d = __uint_as_float(b0 ? s2b : s2a);
-            const float s_ = T.rowP[t & 3][col] + T.rowR[t & 3][col] * vq;
-            e_hi = d + 2.01f * TF32_EPS * s_ * s_;                      // an UPPER bound of the exact energy
-          }
+          for (int i = 0; i < 4; ++i) s4[i] = b2 ? s8[4 + i] : s8[i];
+          const uint32_t s2a = b1 ? s4[2] : s4[0], s2b = b1 ? s4[3] : s4[1];
+          const float d = __uint_as_float(b0 ? s2b : s2a);
+          const float s_ = T.rowP[t & 3][col] + T.rowR[t & 3][col] * vq;
+          const float e_hi = d + 2.01f * TF32_EPS * s_ * s_;              // an UPPER bound of the exact energy
           int pos;
           if (all_pass) {
             pos = (int)(ibase + col);
@@ -240,8 +200,8 @@ __global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity
             pos = blk_base + blk_used++;
           }
           if (pos < p.cap) {
-            my_idx[pos] = IMG ? (int)(ibase + col) : (int)(p.samp_begin + (ibase + col) * p.samp_stride);
-            if (!IMG) my_e[pos] = e_hi;
+            my_idx[pos] = (int)(p.samp_begin + (ibase + col) * p.samp_stride);
+            my_e[pos] = e_hi;
           }
         }
         __syncwarp();      // reconverge before the next aligned wgmma / the barrier arrive
@@ -250,27 +210,8 @@ __global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity
     }
     if (!all_pass && blk_used < RESERVE)
       for (int u = blk_used; u < RESERVE; ++u)
-        if (blk_base + u < p.cap) { my_idx[blk_base + u] = -1; if (!IMG) my_e[blk_base + u] = CUDART_INF_F; }
-  } else if (IMG && warp == 16) {
-    // ============ producer (image path): one thread, one 68 KB bulk copy per tile ============
-    if (lane == 0) {
-      for (int t = 0; t < ntiles; ++t) {
-        const int s = t & 1;
-        mbar_wait(smem_u32(&T.empty[s]), ((t >> 1) & 1) ^ 1);
-        const ImgTile it = img_tile(p, b, tile_of(t));
-        const uint32_t bar = smem_u32(&T.full[s]);
-        mbar_arrive_expect_tx(bar, (uint32_t)OPER_BYTES);
-        // several independent bulk copies per tile: one 68 KB copy is serviced with little memory-level parallelism
-        const uint32_t cb = (uint32_t)OPER_BYTES / (uint32_t)p.img_chunks;
-        const uint32_t dst = smem_u32(Bst + s * OPER_BYTES);
-        for (int c = 0; c < p.img_chunks; ++c) bulk_g2s(dst + c * cb, it.src + (size_t)c * cb, cb, bar);
-        if (p.img_prefetch > 0 && t + p.img_prefetch < ntiles) {       // pull a later tile into L2 ahead of its copy
-          const ImgTile nx = img_tile(p, b, tile_of(t + p.img_prefetch));
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(nx.src), "r"((uint32_t)OPER_BYTES) : "memory");
-        }
-      }
-    }
-  } else if (!IMG && warp < 12) {
+        if (blk_base + u < p.cap) { my_idx[blk_base + u] = -1; my_e[blk_base + u] = CUDART_INF_F; }
+  } else if (warp < 12) {
     // ============ producers: 16 lanes per token row (coalesced 256-B rows), next tile prefetched ============
     const int grp = (warp - 4) >> 2;     // producer group 0 handles even tiles (stage 0), group 1 odd tiles
     const int pt = (tid - 128) & 127;    // 0..127 within the group
@@ -321,7 +262,7 @@ __global__ void __launch_bounds__(IMG ? TC_THREADS_IMG : TC_THREADS, 1) affinity
       for (int j = 0; j < 16; ++j) {
         const int row = r0 + 8 * j;
         float Pn, Rn;
-        store_key_row_operand(Bs, row, c4, kf[j], shr[j], Pn, Rn);      // tc_operand.cuh (shared with the image builder)
+        store_key_row_operand(Bs, row, c4, kf[j], shr[j], Pn, Rn);      // tc_operand.cuh
         if (c4 == 0) {
           T.rowP[t & 3][row] = Pn;
           T.rowR[t & 3][row] = Rn;
@@ -485,22 +426,14 @@ int launch_tc_filter(const TcFilterParams& p, long long B, cudaStream_t st) {
   const size_t smem = tc_filter_smem_bytes();
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done)) {
-    cudaFuncSetAttribute(affinity_tc_filter_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(affinity_tc_filter_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(affinity_tc_filter_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(affinity_tc_filter_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(affinity_tc_filter_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(affinity_tc_filter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   }
   dim3 grid((unsigned)((p.Q + QT - 1) / QT), (unsigned)p.nsplit, (unsigned)B);
-  if (p.use_img) {
-    if (!p.emax_in) return fail(-1, "%s: the image path needs a previous level's thresholds", "affinity_tc_filter_kernel");
-    if (p.dbg_energy)
-      affinity_tc_filter_kernel<true, true><<<grid, TC_THREADS_IMG, smem, st>>>(p);
-    else
-      affinity_tc_filter_kernel<false, true><<<grid, TC_THREADS_IMG, smem, st>>>(p);
-  } else if (p.dbg_energy)
-    affinity_tc_filter_kernel<true, false><<<grid, TC_THREADS, smem, st>>>(p);
+  if (p.dbg_energy)
+    affinity_tc_filter_kernel<true><<<grid, TC_THREADS, smem, st>>>(p);
   else
-    affinity_tc_filter_kernel<false, false><<<grid, TC_THREADS, smem, st>>>(p);
+    affinity_tc_filter_kernel<false><<<grid, TC_THREADS, smem, st>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_cuda_error("affinity_tc_filter_kernel", e);
   return 0;

@@ -1,6 +1,6 @@
-// Shared-memory operand image of the wgmma affinity filter (sm_90a): one definition used by the filter's
-// in-kernel producers (affinity_tc.cu) and by the memory-bank key-image builder (bank.cu), so that a tile fetched
-// with one bulk copy from the bank's precomputed image is bit-identical to a tile converted on the fly.
+// Shared-memory operand layout of the TF32 wgmma affinity filter (sm_90a), written by the filter's in-kernel
+// producers (affinity_tc.cu), which convert fp32 key rows on the fly.  (The bank's precomputed key image is FP16:
+// tc_operand_f16.cuh.)
 //
 // A memory-token tile = 128 rows (tokens) x K = 136 tf32:
 //   4 x [128 rows x 128 B] SWIZZLE_128B K-blocks  : [shr k_c^2 (c = 0..63) | shr k_c (c = 0..63)]
@@ -40,9 +40,9 @@ __device__ __forceinline__ int off_tail(int row, int elem) {     // elem in [0,8
 
 // One token row handled by 16 consecutive lanes (lane c4 = lane & 15 owns channels 4*c4 .. 4*c4+3; all 32 lanes of
 // the warp must call this).  `shr < 0` marks an invalid (out-of-range) row.  Writes the lane's two 16-byte chunks
-// and, from lane c4 == 0, the row's tail (nothing when !do_store); returns the error-bound factors through Pn / Rn.
+// and, from lane c4 == 0, the row's tail; returns the error-bound factors through Pn / Rn.
 __device__ __forceinline__ void store_key_row_operand(unsigned char* tile, int row, int c4, float4 v, float shr,
-                                                      float& Pn, float& Rn, bool do_store = true) {
+                                                      float& Pn, float& Rn) {
   const bool valid = shr >= 0.f;
   const float sh = valid ? shr : 0.f;
   const float4 ln = make_float4(sh * v.x, sh * v.y, sh * v.z, sh * v.w);
@@ -51,17 +51,15 @@ __device__ __forceinline__ void store_key_row_operand(unsigned char* tile, int r
   n2 += __shfl_xor_sync(0xffffffffu, n2, 2);
   n2 += __shfl_xor_sync(0xffffffffu, n2, 4);
   n2 += __shfl_xor_sync(0xffffffffu, n2, 8);
-  if (do_store) {
-    *reinterpret_cast<float4*>(tile + off_main(row, 4 * c4)) = make_float4(ln.x * v.x, ln.y * v.y, ln.z * v.z, ln.w * v.w);
-    *reinterpret_cast<float4*>(tile + off_main(row, 64 + 4 * c4)) = ln;
-  }
+  *reinterpret_cast<float4*>(tile + off_main(row, 4 * c4)) = make_float4(ln.x * v.x, ln.y * v.y, ln.z * v.z, ln.w * v.w);
+  *reinterpret_cast<float4*>(tile + off_main(row, 64 + 4 * c4)) = ln;
   // per-row error-bound factors (rounded up a hair) and the tail block; all 16 lanes of the row hold the
   // same values, lane c4 == 0 stores them (small predicated body, no divergence region)
   Pn = fsqrt_approx(sh * n2) * 1.002f;
   Rn = fsqrt_approx(sh) * 1.002f;
   const float4 t0 = make_float4(sh, valid ? 0.f : TC_BIG_E, sh, -TC_TF32_EPS * Pn * Pn);
   const float4 t1 = make_float4(-2.f * TC_TF32_EPS * Pn * Rn, -TC_TF32_EPS * Rn * Rn, 0.f, 0.f);
-  if (c4 == 0 && do_store) {
+  if (c4 == 0) {
     // tail: [shr, BIG if invalid, shr, -eps P^2 | -2 eps P R, -eps R^2, 0, 0]   x   [b2_hi, 1, b2_lo, 1 | v, v^2, 0, 0]
     *reinterpret_cast<float4*>(tile + off_tail(row, 0)) = t0;
     *reinterpret_cast<float4*>(tile + off_tail(row, 4)) = t1;

@@ -336,7 +336,7 @@ def phase_times(calls_ago: int = 0):
 
 
 def image_level_launches() -> int:
-    """How many filter levels this process has served from a key image (bulk-copy producer) so far."""
+    """How many affinity_topk calls this process has served with the FP16 key-image plan so far."""
     return _entry('cutie_debug_image_level_launches')()
 
 

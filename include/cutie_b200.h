@@ -91,10 +91,11 @@ void cutie_set_tc_min_tokens(int64_t n);
  * exact re-rank) for one of the last 64 calls, measured in situ with events on the caller's stream. */
 void cutie_debug_phase_timing(int enable);
 int cutie_debug_phase_times(int64_t calls_ago, float* out_ms, int max_phases);
-/* Number of filter levels served from a key image so far in this process (diagnostics / tests). */
+/* Number of calls served by the FP16 image plan so far in this process (diagnostics / tests). */
 int64_t cutie_debug_image_level_launches(void);
 /* Test hook: raw TF32 energies E[b,q,n] = -8*S[n,q] computed by the wgmma filter over the whole bank
- * (dbg_energy [B,Q,n_total]); workspace >= cutie_affinity_workspace_bytes(B,Q,n_total,30) + B*Q*n_total*0. */
+ * (dbg_energy [B,Q,n_total]); workspace: the filtered plan's candidate lists and counters followed by two
+ * scratch output arrays, B*Q*(2*16384*4 + 4*4 + 2*32*4) bytes plus the rounding of each of the eight arrays up to 256. */
 int cutie_debug_tc_energy(int num_segments, const void* const* seg_key, const void* const* seg_shrinkage,
                           const int64_t* seg_len, const int64_t* seg_key_bstride, const int64_t* seg_shr_bstride,
                           const float* qk, const float* qe, int64_t B, int64_t Q, int64_t n_total,
@@ -235,10 +236,12 @@ int cutie_prob_to_mask(const float* prob, int64_t plane_stride, int64_t row_stri
  * Replaces the flatten + torch.cat growth of KeyValueMemoryStore.add (kv_memory_store.py:6-16,:136-149). */
 int cutie_bank_append(const float* src, int64_t src_bstride, float* dst_rows, int64_t dst_bstride, int64_t B,
                       int64_t C, int64_t n, void* stream);
-/* Build / refresh the tensor-core operand image for tokens [phys_begin, phys_begin + n) of an arena (key_arena
- * [B, cap, 64], shr_arena [B, cap] token-major; image [B, image_tiles, 9216] floats, image_tiles*128 >= cap; key_mu [B, 64] or NULL: the image holds k - mu.
- * Tile t of the image holds tokens [128 t, 128 t + 128) as [shr k^2 | shr k | shr, 0, shr, -eps P^2, -2 eps P R,
- * -eps R^2, 0, 0] in the filter's shared-memory layout (4 SWIZZLE_128B K-blocks + tail; csrc/tc_operand.cuh).
+/* Build / refresh the FP16 tensor-core operand image for tokens [phys_begin, phys_begin + n) of an arena (key_arena
+ * [B, cap, 64], shr_arena [B, cap] token-major; image [B, image_tiles, 9216] floats = 36864 bytes of f16 operands per
+ * tile, image_tiles*128 >= cap; key_mu [B, 64] or NULL: the image holds k - mu).
+ * Tile t of the image holds tokens [128 t, 128 t + 128) as f16 rows [shr k^2 | shr k | tail] with k centred by mu, in the
+ * FP16 filter's shared-memory layout: 2 SWIZZLE_128B K-blocks of 64 f16 + the 16-element tail block that carries the
+ * error-bound terms (csrc/tc_operand_f16.cuh).
  * Called once per memory frame for the appended tokens -- the per-token part of get_similarity
  * (memory_utils.py:28-36: mk^2, shrinkage scaling) hoisted out of the per-frame read; no reference counterpart. */
 int cutie_bank_key_image(const float* key_arena, int64_t key_bstride, const float* shr_arena, int64_t shr_bstride,
